@@ -115,12 +115,21 @@ __global__ void __launch_bounds__(256) k_msm_count(size_t n, const uint8_t* __re
 }
 
 // ---- MSM stage 2: exclusive scan of the histogram (3 small kernels, 1024 elements per block) -------
+// Column y = blockIdx.y scans the bucket sizes after y affine pair-tree rounds, ceil(counts / 2^y) (msm_affine.cuh); column 0
+// (the histogram itself) goes to offs, column y >= 1 to offs_rounds + (y - 1) (total + 1).  Block totals: bsum + 1024 y.
+B2K_D uint32_t* scan_column(uint32_t total, uint32_t* offs, uint32_t* offs_rounds, uint32_t y) {
+  return y == 0 ? offs : offs_rounds + (size_t)(y - 1) * (total + 1);
+}
 // pass A: per-block exclusive scan + block totals
 static __global__ void __launch_bounds__(1024) k_scan_blocks(uint32_t total, const uint32_t* __restrict__ counts,
-                                                      uint32_t* __restrict__ offs, uint32_t* __restrict__ bsum) {
+                                                      uint32_t* __restrict__ offs, uint32_t* __restrict__ offs_rounds,
+                                                      uint32_t* __restrict__ bsum) {
   __shared__ uint32_t wsum[32];
+  const uint32_t y = blockIdx.y;
+  offs = scan_column(total, offs, offs_rounds, y);
+  bsum += 1024u * y;
   uint32_t i = blockIdx.x * 1024u + threadIdx.x;
-  uint32_t v = (i < total) ? counts[i] : 0u;
+  uint32_t v = (i < total) ? pt_round_count(counts[i], y) : 0u;
   uint32_t x = v;
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -145,8 +154,10 @@ static __global__ void __launch_bounds__(1024) k_scan_blocks(uint32_t total, con
 }
 // pass B: exclusive scan of the block totals (<= 1024 blocks), grand total to offs[total]
 static __global__ void __launch_bounds__(1024) k_scan_tops(uint32_t nblocks, uint32_t total, uint32_t* __restrict__ bsum,
-                                                    uint32_t* __restrict__ offs) {
+                                                    uint32_t* __restrict__ offs, uint32_t* __restrict__ offs_rounds) {
   __shared__ uint32_t sm[1024];
+  offs = scan_column(total, offs, offs_rounds, blockIdx.y);
+  bsum += 1024u * blockIdx.y;
   int tid = threadIdx.x;
   uint32_t v = ((uint32_t)tid < nblocks) ? bsum[tid] : 0u;
   sm[tid] = v;
@@ -160,14 +171,17 @@ static __global__ void __launch_bounds__(1024) k_scan_tops(uint32_t nblocks, uin
   if ((uint32_t)tid < nblocks) bsum[tid] = sm[tid] - v;
   if (tid == 1023) offs[total] = sm[1023];
 }
-// pass C: add block offsets, duplicate into the scatter cursor
+// pass C: add block offsets, duplicate column 0 into the scatter cursor
 static __global__ void __launch_bounds__(1024) k_scan_finish(uint32_t total, const uint32_t* __restrict__ bsum,
-                                                      uint32_t* __restrict__ offs, uint32_t* __restrict__ cursor) {
+                                                      uint32_t* __restrict__ offs, uint32_t* __restrict__ offs_rounds,
+                                                      uint32_t* __restrict__ cursor) {
+  const uint32_t y = blockIdx.y;
+  offs = scan_column(total, offs, offs_rounds, y);
   uint32_t i = blockIdx.x * 1024u + threadIdx.x;
   if (i >= total) return;
-  uint32_t o = offs[i] + bsum[blockIdx.x];
+  uint32_t o = offs[i] + bsum[1024u * y + blockIdx.x];
   offs[i] = o;
-  cursor[i] = o;
+  if (y == 0) cursor[i] = o;
 }
 
 // ---- MSM stage 3: counting-sort scatter ----------------------------------------------------------
@@ -227,13 +241,7 @@ __global__ void __launch_bounds__(128, MINB) k_msm_accumulate_slices_direct(uint
   msm_accumulate_slice<CV, true>(j, L, total, pts, offs, nullptr, buckets, spart);
 }
 
-// ---- MSM stage 4a: affine pair-tree rounds (msm_affine.cuh) ---------------------------------------------------
-// operand count of every bucket after one round
-static __global__ void __launch_bounds__(256) k_pt_counts(uint32_t total, const uint32_t* __restrict__ offs_in,
-                                                          uint32_t* __restrict__ counts) {
-  uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g < total) counts[g] = (offs_in[g + 1] - offs_in[g] + 1u) >> 1;
-}
+// ---- MSM stage 4a: affine pair-tree rounds (msm_affine.cuh; bucket offsets of every round from the stage-2 scan) -------
 // one thread = B consecutive outputs: B batched affine additions around one inversion
 template <class CV, bool FIRST>
 __global__ void __launch_bounds__(128, 4) k_msm_pairtree_round(uint32_t B, uint32_t total,

@@ -6,8 +6,11 @@
 // element + one shared inversion), i.e. 6 products per addition -- if independent additions are available.  The serial
 // "acc += P" of a bucket is not; a pair tree is: one ROUND replaces the k sorted operands of every bucket by the
 // ceil(k/2) sums of neighbouring pairs (an odd last operand is carried over), and the rounds' outputs are again affine
-// points grouped by bucket.  R rounds shrink the entry list 2^R-fold (trading extra HBM traffic, which the pass has to
-// spare, for 40 % fewer products); the XYZZ slices of msm.cuh finish what is left.
+// points grouped by bucket.  R rounds shrink the entry list 2^R-fold, for 40 % fewer products but extra HBM traffic: each
+// round writes its outputs and a prefix-product array and reads them back.  On H100 (3.35 TB/s) that traffic costs about
+// what the saved products gain (DESIGN.md section 4), so the automatic plan runs no rounds there (msm_host.cuh: affine_plan);
+// the XYZZ slices of msm.cuh finish what the rounds leave.  A bucket of k operands holds ceil(k / 2^r) after r rounds, so the
+// bucket offsets of every round follow from the main histogram (pt_round_count; one multi-column scan, kernels.cuh).
 //
 // One thread owns B consecutive OUTPUT positions of a round:
 //   forward : fetch the two operands, classify, d_j = x2 - x1 (2 y1 for a doubling, 1 when nothing is to invert),
@@ -41,6 +44,9 @@ template <class C> B2K_D void f_inv_bg(Fp2<C>& r, const Fp2<C>& a) {
 
 constexpr int PT_MAXB = 64;     // outputs per thread (length of the prefix-product array in local memory)
 enum : int { PT_COPY1 = 0, PT_COPY2 = 1, PT_ADD = 2, PT_DBL = 3, PT_INF = 4 };
+
+// operands of a bucket of k after r rounds: ceil(k / 2^r) (= r halvings with the odd operand carried over)
+B2K_D uint32_t pt_round_count(uint32_t k, uint32_t r) { return (k >> r) + ((k & ((1u << r) - 1u)) != 0u); }
 
 // operands of the output at input position a (pairs start at even offsets of the bucket's run [.., end))
 template <class CV, bool FIRST>
@@ -127,7 +133,9 @@ B2K_D void msm_pairtree_round(uint32_t t, uint32_t B, uint32_t total, const Affi
 // inlined products) resident at once and runs them all at the register budget of the widest; split, every phase has
 // compact code and its own occupancy, the prefix products travel through a coalesced global array pre[j * T + t] and the
 // running product / its inverse through accs[t].  The forward pass reads only the x coordinates (dx is all it needs;
-// x = 0 or dx = 0 fall back to the full classification).
+// x = 0 or dx = 0 fall back to the full classification).  (Inverting at the end of the forward kernel instead was measured
+// on H100: the one-wave forward grid reaches its inversions together, so they stay a tail, and the forward loop compiles
+// worse next to them -- slower than the separate pass.)
 template <class CV, bool FIRST>
 B2K_D void pt_denominator(typename CV::F& d, const Affine<typename CV::F>* in, const uint32_t* entries, uint32_t a, uint32_t end) {
   using F = typename CV::F;

@@ -164,13 +164,12 @@ inline AffinePlan affine_plan(const b2k_ctx* ctx, size_t n, const MsmPlan& pl) {
   if (!AffineTraits<CV>::enabled || ctx->use_v1 || ctx->msm_groups > 1) return ap;
   const size_t total = (size_t)pl.W * pl.nb;
   int R = ctx->affine_rounds;
-  if (R < 0) {                          // automatic: big problems only; measured best at C2 (64 operands per bucket): 3 rounds --
-    R = 0;                              // later, smaller rounds no longer fill the chip and the XYZZ slices take over
-    if (ap.bound[0] >= (size_t(1) << 20)) {
-      const size_t avg = ap.bound[0] / total;
-      while (R < PT_MAX_ROUNDS && (avg >> R) >= 16) R++;
-    }
-  }
+  // automatic: no rounds.  Measured on H100 at C2 (64 operands per bucket; profiles/h100_kernels_*.txt, h100_rounds_*.txt):
+  // every round costs about the XYZZ slice time it saves (round 0: 0.94 + 0.14 + 2.38 ms of forward / inversion / backward
+  // against 3.37 ms of slices), so 0..3 rounds land within 1.5 % of each other in kernel time, none ahead of R = 0, and no
+  // batch width 16..256 beat the automatic one; without rounds the MSM also needs ~1.6 GB less scratch (round outputs and
+  // prefix products).  b2k_set_msm_affine still forces them.
+  if (R < 0) R = 0;
   if (R > PT_MAX_ROUNDS) R = PT_MAX_ROUNDS;
   ap.R = R;
   for (int r = 0; r < R; r++) {
@@ -221,9 +220,9 @@ size_t msm_scratch_bytes(const b2k_ctx* ctx, size_t n, const MsmPlan& pl) {
     if (sa > smax) smax = sa;
   }
   b += pad256(2 * smax * sizeof(Xyzz<F>));        // slice partials (worst case: smallest automatic L)
-  b += pad256((total + 1) * 4) + pad256(4096);    // big-bucket list, block sums
+  b += pad256((total + 1) * 4) + pad256(4096 * (size_t)(1 + ap.R));   // big-bucket list, block sums (one page per scanned column)
   if (ap.R > 0) {
-    b += 2 * pad256((total + 1) * 4);             // bucket offsets of the rounds (ping-pong)
+    b += pad256((size_t)ap.R * (total + 1) * 4);  // bucket offsets after each round
     b += pad256(ap.bound[1] * sizeof(Affine<F>));
     if (ap.R > 1) b += pad256(ap.bound[2] * sizeof(Affine<F>));
     if (ctx->affine_split) b += pad256(ap.pre_elems * sizeof(F)) + pad256((size_t)ap.max_T * sizeof(F));
@@ -272,19 +271,19 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
   const uint32_t sa = ap.R > 0 ? (uint32_t)((ap.bound[ap.R] + La - 1) / La) + 1 : 0;      // slices after the affine rounds
   auto* spart = arena_take<Xyzz<F>>(ctx, 2 * (size_t)(sa > smax ? sa : smax));
   auto* big_list = arena_take<uint32_t>(ctx, total + 1);
-  auto* bsum = arena_take<uint32_t>(ctx, 1024);
+  auto* bsum = arena_take<uint32_t>(ctx, 1024 * (size_t)(1 + ap.R));   // block sums of the scan, 1024 words per column
   if (!spart || !big_list || !bsum || total > 1024u * 1024u) {
     ctx->err = "scratch arena too small / too many buckets";
     return B2K_ERR_ARG;
   }
-  uint32_t* offs_rt[2] = {nullptr, nullptr};
+  // bucket offsets after round r + 1: offs_rt + r (total + 1), written by the stage-2 scan (columns 1..R)
+  uint32_t* offs_rt = nullptr;
   Affine<F>* aff_rt[2] = {nullptr, nullptr};
   if (ap.R > 0) {
-    offs_rt[0] = arena_take<uint32_t>(ctx, total + 1);
-    offs_rt[1] = arena_take<uint32_t>(ctx, total + 1);
+    offs_rt = arena_take<uint32_t>(ctx, (size_t)ap.R * (total + 1));
     aff_rt[0] = arena_take<Affine<F>>(ctx, ap.bound[1]);
     if (ap.R > 1) aff_rt[1] = arena_take<Affine<F>>(ctx, ap.bound[2]);
-    if (!offs_rt[0] || !offs_rt[1] || !aff_rt[0] || (ap.R > 1 && !aff_rt[1])) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
+    if (!offs_rt || !aff_rt[0] || (ap.R > 1 && !aff_rt[1])) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
   }
   F* pt_pre = nullptr;
   F* pt_accs = nullptr;
@@ -331,9 +330,12 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
   CK(cudaEventRecord(ctx->ev[1], st));
   k_msm_count<CV><<<gb_n, 256, 0, st>>>(n, d_scalars, pl, counts, ctx->d_flags); nl++;
   CK(cudaEventRecord(ctx->ev[2], st));
-  k_scan_blocks<<<sblocks, 1024, 0, st>>>((uint32_t)total, counts, offs, bsum);
-  k_scan_tops<<<1, 1024, 0, st>>>(sblocks, (uint32_t)total, bsum, offs);
-  k_scan_finish<<<sblocks, 1024, 0, st>>>((uint32_t)total, bsum, offs, cursor); nl += 3;
+  {
+    const dim3 cols(sblocks, 1 + ap.R), tops(1, 1 + ap.R);     // the histogram + the bucket sizes after each affine round
+    k_scan_blocks<<<cols, 1024, 0, st>>>((uint32_t)total, counts, offs, offs_rt, bsum);
+    k_scan_tops<<<tops, 1024, 0, st>>>(sblocks, (uint32_t)total, bsum, offs, offs_rt);
+    k_scan_finish<<<cols, 1024, 0, st>>>((uint32_t)total, bsum, offs, offs_rt, cursor); nl += 3;
+  }
   CK(cudaEventRecord(ctx->ev[3], st));
   k_msm_scatter<CV><<<gb_n, 256, 0, st>>>(n, d_scalars, pl, cursor, entries); nl++;
   const int G = (!ext_buckets && !ctx->use_v1 && ctx->msm_groups > 1 && pl.W >= 2 * ctx->msm_groups && ctx->stream2) ? ctx->msm_groups : 1;
@@ -384,12 +386,8 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
         const uint32_t* offs_cur = offs;
         const Affine<F>* in_cur = pts;
         for (int r = 0; r < ap.R; r++) {
-          uint32_t* offs_nxt = offs_rt[r & 1];
+          const uint32_t* offs_nxt = offs_rt + (size_t)r * (total + 1);
           Affine<F>* out = aff_rt[r & 1];
-          k_pt_counts<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint32_t)total, offs_cur, counts);
-          k_scan_blocks<<<sblocks, 1024, 0, st>>>((uint32_t)total, counts, offs_nxt, bsum);
-          k_scan_tops<<<1, 1024, 0, st>>>(sblocks, (uint32_t)total, bsum, offs_nxt);
-          k_scan_finish<<<sblocks, 1024, 0, st>>>((uint32_t)total, bsum, offs_nxt, cursor);
           const unsigned grid = ap.T[r] / 128;
           if (ctx->affine_split) {
             constexpr size_t fstage_bytes = 128 * 4 * sizeof(F);              // two 2-coordinate buffers per thread (24 KB for G1)
@@ -416,11 +414,11 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
               if (r == 0) k_pt_backward<CV, true><<<grid, 128, 0, st>>>(ap.B[r], (uint32_t)total, in_cur, entries, offs_cur, offs_nxt, pt_pre, pt_accs, out);
               else k_pt_backward<CV, false><<<grid, 128, 0, st>>>(ap.B[r], (uint32_t)total, in_cur, nullptr, offs_cur, offs_nxt, pt_pre, pt_accs, out);
             }
-            nl += 7;
+            nl += 3;
           } else {
             if (r == 0) k_msm_pairtree_round<CV, true><<<grid, 128, 0, st>>>(ap.B[r], (uint32_t)total, in_cur, entries, offs_cur, offs_nxt, out);
             else k_msm_pairtree_round<CV, false><<<grid, 128, 0, st>>>(ap.B[r], (uint32_t)total, in_cur, nullptr, offs_cur, offs_nxt, out);
-            nl += 5;
+            nl += 1;
           }
           offs_cur = offs_nxt;
           in_cur = out;

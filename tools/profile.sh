@@ -15,7 +15,7 @@ python tools/summarize_launches.py gpurun_out/launches_${TAG}.csv > gpurun_out/$
 # the bucket-accumulate pass of ONE MSM, once: the three kernels of every affine pair-tree round + the XYZZ slices
 # (NK = 3 R + 1 launches per MSM; skip the first 3 MSMs)
 NK=${B2K_PROFILE_PASS_KERNELS:-10}
-ncu --set full --clock-control none --import-source on -k "regex:k_pt_forward|k_pt_invert|k_pt_backward|k_msm_accumulate_slices" -s $((3 * NK)) -c $NK \
+ncu --set full --clock-control none --import-source on -k "regex:k_pt_forward|k_pt_backward|k_msm_accumulate_slices" -s $((3 * NK)) -c $NK \
     -o gpurun_out/accumulate_${TAG} -f python bench.py --steps 1 --warmup 3 --contexts 1 > gpurun_out/ncu_full_${TAG}.log 2>&1
 # gpurun_out/ travels back only below 64 MiB: keep the text pages, drop the report
 ncu -i gpurun_out/accumulate_${TAG}.ncu-rep --page details > gpurun_out/${TAG}_accumulate_ncu_details.txt 2>&1
