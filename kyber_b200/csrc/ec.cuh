@@ -160,7 +160,8 @@ B2K_D void xyzz_dbl(Xyzz<F>& r, const Xyzz<F>& p) {
 template <class F>
 B2K_NI void xyzz_dbl_rare(Xyzz<F>& r, const Xyzz<F>& p) { xyzz_dbl(r, p); }
 
-// madd-2008-s: 8M + 2S; q given affine, optionally negated (signed-digit buckets)
+// madd-2008-s: 8M + 2S; q given affine, optionally negated (signed-digit buckets).  Over Fp, Y3 = R (Q - X3) - Y1 PPP is one
+// sum of two products (f_mul_sub); Fp2 keeps two products: that form of Y3 tripped an illegal access in the G2 MSM on sm_90a
 template <class F>
 B2K_D void xyzz_madd(Xyzz<F>& r, const Xyzz<F>& p, const Affine<F>& q, bool negate) {
   if (aff_is_inf(q)) { r = p; return; }
@@ -183,15 +184,20 @@ B2K_D void xyzz_madd(Xyzz<F>& r, const Xyzz<F>& p, const Affine<F>& q, bool nega
   f_mul(PPP, P, PP);
   f_mul(Q, p.X, PP);
   f_sqr(U2, R); f_sub(U2, U2, PPP); f_sub(U2, U2, Q); f_sub(U2, U2, Q);   // X3
-  f_sub(Q, Q, U2); f_mul(Q, R, Q);
-  f_mul(S2, p.Y, PPP);
-  f_sub(r.Y, Q, S2);
+  f_sub(Q, Q, U2);
+  if constexpr (f_is_base<F>) {
+    f_mul_sub(r.Y, R, Q, p.Y, PPP, S2);                                    // R (Q - X3) - Y1 PPP
+  } else {
+    f_mul(Q, R, Q);
+    f_mul(S2, p.Y, PPP);
+    f_sub(r.Y, Q, S2);
+  }
   r.X = U2;
   f_mul(r.ZZ, p.ZZ, PP);
   f_mul(r.ZZZ, p.ZZZ, PPP);
 }
 
-// add-2008-s: 12M + 2S
+// add-2008-s: 12M + 2S (Y3 likewise over Fp)
 template <class F>
 B2K_D void xyzz_add(Xyzz<F>& r, const Xyzz<F>& p, const Xyzz<F>& q) {
   if (xyzz_is_inf(q)) { r = p; return; }
@@ -211,11 +217,18 @@ B2K_D void xyzz_add(Xyzz<F>& r, const Xyzz<F>& p, const Xyzz<F>& q) {
   f_mul(PPP, P, PP);
   f_mul(Q, U1, PP);
   f_sqr(U2, R); f_sub(U2, U2, PPP); f_sub(U2, U2, Q); f_sub(U2, U2, Q);   // X3
-  f_sub(Q, Q, U2); f_mul(Q, R, Q);
-  f_mul(S1, S1, PPP);
-  f_mul(U1, p.ZZ, q.ZZ);
-  f_mul(S2, p.ZZZ, q.ZZZ);
-  f_sub(r.Y, Q, S1);
+  if constexpr (f_is_base<F>) {
+    f_sub(Q, Q, U2);
+    f_mul(U1, p.ZZ, q.ZZ);
+    f_mul(S2, p.ZZZ, q.ZZZ);
+    f_mul_sub(r.Y, R, Q, S1, PPP, S1);                                     // R (Q - X3) - S1 PPP
+  } else {
+    f_sub(Q, Q, U2); f_mul(Q, R, Q);
+    f_mul(S1, S1, PPP);
+    f_mul(U1, p.ZZ, q.ZZ);
+    f_mul(S2, p.ZZZ, q.ZZZ);
+    f_sub(r.Y, Q, S1);
+  }
   r.X = U2;
   f_mul(r.ZZ, U1, PP);
   f_mul(r.ZZZ, S2, PPP);

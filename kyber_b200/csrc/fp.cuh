@@ -226,6 +226,97 @@ B2K_D void redc_wide(uint32_t* r, const uint32_t* t) {
   r[N - 1] = ptx::addc(ev[N - 1], t[2 * N - 1]);
 }
 
+// ---- one-level subtractive Karatsuba wide products (the sum of two products of the XYZZ formulas, ec.cuh) -------------------
+// With H = N/2, B = 2^(32H), a = a0 + a1 B, b = b0 + b1 B, z0 = a0 b0, z2 = a1 b1:
+//   a b = z0 + (z0 + z2 - (a0 - a1)(b0 - b1)) B + z2 B^2,
+// where (a0 - a1)(b0 - b1) = +-|a0 - a1| |b0 - b1| by the signs of the two differences.  3 H^2 = 3/4 N^2 multiply-adds
+// instead of N^2, for ~110 additions and selects that run on the integer ALU, which the FMA-heavy pipe leaves idle.  The
+// halves go through wide_mul<H>, whose rows pair limbs, so H must be even: N = 12 and 8.  N = 10 (bn256) keeps the
+// schoolbook wide_mul.
+
+// d = |x0 - x1| for the two H-limb halves of x; returns all-ones if x0 < x1, else 0 (also when x0 = x1: d = 0)
+template <int H>
+B2K_D uint32_t half_absdiff(uint32_t* d, const uint32_t* x) {
+  d[0] = ptx::sub_cc(x[0], x[H]);
+#pragma unroll
+  for (int j = 1; j < H; j++) d[j] = ptx::subc_cc(x[j], x[H + j]);
+  const uint32_t neg = ptx::subc(0, 0);
+  d[0] = ptx::add_cc(d[0] ^ neg, neg & 1u);          // two's complement negation when negative: (d ^ ~0) + 1
+#pragma unroll
+  for (int j = 1; j < H - 1; j++) d[j] = ptx::addc_cc(d[j] ^ neg, 0);
+  d[H - 1] = ptx::addc(d[H - 1] ^ neg, 0);
+  return neg;
+}
+
+// One Karatsuba term a b into (t, mid), with H even.  FIRST: t = z0 + z2 B^2 and mid = z0 + z2 -+ |a0 - a1| |b0 - b1|; later terms
+// add to both, z2 before z0, so that every partial sum stays below the final one and the carry out of the top limb is 0.
+// mid holds N + 1 limbs modulo 2^(32(N+1)): it starts from the signed |..||..|, so only one half-product and the half-operand
+// pair it needs are live at a time; a term's middle part lies in [0, 2^(64H+1)), two of them below 2^(32(N+1)).
+template <int N, bool FIRST>
+B2K_D void kara_term(uint32_t* t, uint32_t* mid, const uint32_t* a, const uint32_t* b) {
+  constexpr int H = N / 2;
+  uint32_t z[N], da[H], db[H];
+  const uint32_t sa = half_absdiff<H>(da, a), sb = half_absdiff<H>(db, b);
+  wide_mul<H>(z, da, db);
+  const uint32_t m = ~(sa ^ sb);                      // all-ones: (a0 - a1)(b0 - b1) >= 0, so the middle part subtracts it
+  ptx::add_cc(m, m & 1u);                             // carry-in 1 for the two's complement (~0 + 1 carries, 0 + 0 does not)
+#pragma unroll
+  for (int j = 0; j < N; j++) mid[j] = ptx::addc_cc(FIRST ? 0 : mid[j], z[j] ^ m);
+  mid[N] = ptx::addc(FIRST ? 0 : mid[N], m);
+  wide_mul<H>(z, a + H, b + H);                       // z2
+  if (FIRST) {
+#pragma unroll
+    for (int j = 0; j < N; j++) t[N + j] = z[j];
+  } else {
+    t[N] = ptx::add_cc(t[N], z[0]);
+#pragma unroll
+    for (int j = 1; j < N - 1; j++) t[N + j] = ptx::addc_cc(t[N + j], z[j]);
+    t[2 * N - 1] = ptx::addc(t[2 * N - 1], z[N - 1]);
+  }
+  mid[0] = ptx::add_cc(mid[0], z[0]);
+#pragma unroll
+  for (int j = 1; j < N; j++) mid[j] = ptx::addc_cc(mid[j], z[j]);
+  mid[N] = ptx::addc(mid[N], 0);
+  wide_mul<H>(z, a, b);                               // z0
+  if (FIRST) {
+#pragma unroll
+    for (int j = 0; j < N; j++) t[j] = z[j];
+  } else {
+    t[0] = ptx::add_cc(t[0], z[0]);
+#pragma unroll
+    for (int j = 1; j < N; j++) t[j] = ptx::addc_cc(t[j], z[j]);
+#pragma unroll
+    for (int j = N; j < 2 * N - 1; j++) t[j] = ptx::addc_cc(t[j], 0);
+    t[2 * N - 1] = ptx::addc(t[2 * N - 1], 0);
+  }
+  mid[0] = ptx::add_cc(mid[0], z[0]);
+#pragma unroll
+  for (int j = 1; j < N; j++) mid[j] = ptx::addc_cc(mid[j], z[j]);
+  mid[N] = ptx::addc(mid[N], 0);
+}
+
+// t += mid B
+template <int N>
+B2K_D void kara_finish(uint32_t* t, const uint32_t* mid) {
+  constexpr int H = N / 2;
+  t[H] = ptx::add_cc(t[H], mid[0]);
+#pragma unroll
+  for (int j = 1; j <= N; j++) t[H + j] = ptx::addc_cc(t[H + j], mid[j]);
+#pragma unroll
+  for (int k = H + N + 1; k < 2 * N - 1; k++) t[k] = ptx::addc_cc(t[k], 0);
+  t[2 * N - 1] = ptx::addc(t[2 * N - 1], 0);
+}
+
+// t[0..2N) = a * b + c * d for a sum below 2^(64N); the two middle parts share one mid and one shifted addition
+template <int N>
+B2K_D void wide_mul_kara_sum2(uint32_t* t, const uint32_t* a, const uint32_t* b, const uint32_t* c, const uint32_t* d) {
+  static_assert(N % 4 == 0, "Karatsuba halves of an even limb count");
+  uint32_t mid[N + 1];
+  kara_term<N, true>(t, mid, a, b);
+  kara_term<N, false>(t, mid, c, d);
+  kara_finish<N>(t, mid);
+}
+
 }  // namespace detail
 
 // ---- comparison / conditional subtraction ---------------------------------------------------
@@ -277,6 +368,28 @@ B2K_D void fp_sqr_inl(Fp<C>& r, const Fp<C>& a) {
   for (int j = 0; j < N; j++) r.v[j] = u[j];
 }
 
+
+// (a b + c d) R^-1 with ONE reduction: both products accumulate into one wide buffer, a b + c d < 2 p^2 < p 2^(32N) for
+// operands below p (2 p < 2^(32N) for every field here), which is what redc_wide needs.  N = 10 (bn256), whose halves would
+// have an odd limb count, adds two CIOS products instead.
+template <class C>
+B2K_D void fp_mul_sum2_inl(Fp<C>& r, const Fp<C>& a, const Fp<C>& b, const Fp<C>& c, const Fp<C>& d) {
+  constexpr int N = C::N;
+  if constexpr (N % 4 != 0) {
+    Fp<C> ab, cd;
+    fp_mul_inl(ab, a, b);
+    fp_mul_inl(cd, c, d);
+    fp_add(r, ab, cd);
+  } else {
+    uint32_t t[2 * N], u[N];
+    detail::wide_mul_kara_sum2<N>(t, a.v, b.v, c.v, d.v);
+    detail::redc_wide<C>(u, t);
+    fp_reduce_once<C>(u);
+#pragma unroll
+    for (int j = 0; j < N; j++) r.v[j] = u[j];
+  }
+}
+
 // ---- code layout of the two products ----------------------------------------------------------------------------------------
 // Default: fully inlined at every use (a 381-bit product is ~330 instructions = 5.3 KB of SASS).  A translation unit compiled
 // with B2K_COMPACT_FIELD gets ONE out-of-line copy of each product instead, called BY VALUE: nvcc passes the 2 x N operand
@@ -295,6 +408,16 @@ template <class C> B2K_D void fp_sqr(Fp<C>& r, const Fp<C>& a) { r = fp_sqr_v<C>
 #else
 template <class C> B2K_D void fp_mul(Fp<C>& r, const Fp<C>& a, const Fp<C>& b) { fp_mul_inl(r, a, b); }
 template <class C> B2K_D void fp_sqr(Fp<C>& r, const Fp<C>& a) { fp_sqr_inl(r, a); }
+#endif
+
+// the sum of two products (fp_mul_sum2_inl), same layout rule; operands and result by value in the compact layout
+#ifdef B2K_COMPACT_FIELD
+template <class C> B2K_NI Fp<C> fp_mul_sum2_v(Fp<C> a, Fp<C> b, Fp<C> c, Fp<C> d) { Fp<C> r; fp_mul_sum2_inl(r, a, b, c, d); return r; }
+template <class C>
+B2K_D void fp_mul_sum2(Fp<C>& r, const Fp<C>& a, const Fp<C>& b, const Fp<C>& c, const Fp<C>& d) { r = fp_mul_sum2_v<C>(a, b, c, d); }
+#else
+template <class C>
+B2K_D void fp_mul_sum2(Fp<C>& r, const Fp<C>& a, const Fp<C>& b, const Fp<C>& c, const Fp<C>& d) { fp_mul_sum2_inl(r, a, b, c, d); }
 #endif
 
 // out-of-line copies for code that is too large to inline a 300-instruction product at every use

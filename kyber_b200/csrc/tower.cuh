@@ -180,6 +180,15 @@ template <class C> B2K_D void f_mul_i(Fp<C>& r, const Fp<C>& a, const Fp<C>& b) 
 template <class C> B2K_D void f_sqr_i(Fp<C>& r, const Fp<C>& a) { fp_sqr_i(r, a); }
 template <class C> B2K_D void f_mul_i(Fp2<C>& r, const Fp2<C>& a, const Fp2<C>& b) { fp2_mul(r, a, b); }
 template <class C> B2K_D void f_sqr_i(Fp2<C>& r, const Fp2<C>& a) { fp2_sqr(r, a); }
+// r = a b - c d for the Y3 of the XYZZ additions over Fp (ec.cuh): one reduction for both products, (a b + (p - c) d) R^-1
+// (fp.cuh, fp_mul_sum2); t is scratch.  Fp2 (G2) and the probe fields keep two products and a subtraction (f_is_base).
+template <class F> inline constexpr bool f_is_base = false;
+template <class C> inline constexpr bool f_is_base<Fp<C>> = true;
+template <class C>
+B2K_D void f_mul_sub(Fp<C>& r, const Fp<C>& a, const Fp<C>& b, const Fp<C>& c, const Fp<C>& d, Fp<C>& t) {
+  fp_neg(t, c);
+  fp_mul_sum2(r, a, b, t, d);
+}
 template <class C> B2K_D void f_add(Fp2<C>& r, const Fp2<C>& a, const Fp2<C>& b) { fp2_add(r, a, b); }
 template <class C> B2K_D void f_sub(Fp2<C>& r, const Fp2<C>& a, const Fp2<C>& b) { fp2_sub(r, a, b); }
 template <class C> B2K_D void f_mul(Fp2<C>& r, const Fp2<C>& a, const Fp2<C>& b) { fp2_mul(r, a, b); }

@@ -19,6 +19,7 @@ WATCH = {  # kernel name fragment -> max instructions of its largest 12-limb pro
     "k_coop_pairing_check": 420, "k_coop_pairE": 420,                                # the cooperative ones
     "k_msm_accumulate_slicesINS_8Bls381G2": 420, "k_msm_reduce_l1INS_8Bls381G2": 420, "k_msm_accumulateINS_8Bls381G2": 420,   # b2k_g2.o
     "k_msm_accumulate_slices_directINS_8Bls381G1": 420, "k_pt_backwardINS_8Bls381G1": 420,                                  # b2k_api.o
+    "k_msm_accumulate_slicesINS_8Bls381G1ELi3": 420,                                 # the slice kernel the automatic plan runs
 }
 
 

@@ -6,12 +6,15 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "fp.cuh"
+#include "fp_kara.cuh"
 #include "fp29.cuh"
 #include "constants.cuh"
 using namespace b2k;
 using F = Fp<Bls381Fp>;
 
-template <int CHAINS, bool NOINLINE>
+// FORM 0: CIOS product (fp_mul), 1: Karatsuba wide product + redc_wide (fp_kara.cuh: fp_mul_k_inl),
+//      2: sum of two products with one reduction (fp_kara.cuh: fp_mul_sum2_inl; counted as two products)
+template <int CHAINS, bool NOINLINE, int FORM = 0>
 __global__ void __launch_bounds__(128) k_mul(int iters, uint32_t* out, uint32_t seed) {
   F a[CHAINS], b;
 #pragma unroll
@@ -24,7 +27,9 @@ __global__ void __launch_bounds__(128) k_mul(int iters, uint32_t* out, uint32_t 
   for (int i = 0; i < iters; i++) {
 #pragma unroll
     for (int c = 0; c < CHAINS; c++) {
-      if (NOINLINE) fp_mul_c(a[c], a[c], b);
+      if (FORM == 1) fp_mul_k_inl(a[c], a[c], b);
+      else if (FORM == 2) fp_mul_sum2_inl(a[c], a[c], b, b, a[c]);
+      else if (NOINLINE) fp_mul_c(a[c], a[c], b);
       else fp_mul(a[c], a[c], b);
     }
   }
@@ -83,20 +88,20 @@ static void run29(const char* name, int blocks_per_sm, int sms, int clk_khz, uin
   (void)clk_khz;
 }
 
-template <int CHAINS, bool NI>
+template <int CHAINS, bool NI, int FORM = 0>
 static void run(const char* name, int blocks_per_sm, int sms, int clk_khz, uint32_t* out) {
   const int iters = 2048;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  k_mul<CHAINS, NI><<<sms * blocks_per_sm, 128>>>(64, out, 5);
+  k_mul<CHAINS, NI, FORM><<<sms * blocks_per_sm, 128>>>(64, out, 5);
   cudaDeviceSynchronize();
   cudaEventRecord(e0);
-  k_mul<CHAINS, NI><<<sms * blocks_per_sm, 128>>>(iters, out, 9);
+  k_mul<CHAINS, NI, FORM><<<sms * blocks_per_sm, 128>>>(iters, out, 9);
   cudaEventRecord(e1);
   cudaEventSynchronize(e1);
   float ms;
   cudaEventElapsedTime(&ms, e0, e1);
-  const double muls = (double)sms * blocks_per_sm * 128 * iters * CHAINS;
+  const double muls = (double)sms * blocks_per_sm * 128 * iters * CHAINS * (FORM == 2 ? 2 : 1);
   const double per_s = muls / (ms * 1e-3);
   const double imad_clk_sm = muls * 302.0 / (ms * 1e-3 * clk_khz * 1e3) / sms;
   printf("%-28s blocks/SM %d  %8.3f ms  %.3e fp_mul/s  %5.1f IMAD-class thread-instr/clk/SM\n", name, blocks_per_sm, ms, per_s, imad_clk_sm);
@@ -110,7 +115,12 @@ int main() {
   uint32_t* out;
   cudaMalloc(&out, 8);
   const int sms = p.multiProcessorCount;
+  printf("%s, %d SMs, max SM clock %d MHz\n", p.name, sms, clk / 1000);
   for (int bps : {2, 4, 8}) {
+    run<1, false, 1>("karatsuba, 1 chain", bps, sms, clk, out);
+    run<2, false, 1>("karatsuba, 2 chains", bps, sms, clk, out);
+    run<1, false, 2>("sum of two, 1 chain", bps, sms, clk, out);
+    run<2, false, 2>("sum of two, 2 chains", bps, sms, clk, out);
     run<1, false>("inline, 1 chain", bps, sms, clk, out);
     run<2, false>("inline, 2 chains", bps, sms, clk, out);
     run<4, false>("inline, 4 chains", bps, sms, clk, out);
