@@ -97,8 +97,9 @@ static void emul_mul_batch_w4(size_t n, const uint8_t* scalars, const uint8_t* p
   }
 }
 
-static MsmPlan emul_plan(int c, int m) {
-  MsmPlan pl; pl.c = c; pl.W = (256 + c - 1) / c; pl.nb = 1 << (c - 1); pl.m = m;
+// the device's plan (msm_host.cuh: make_plan): signed-digit recoding needs windows for scalar_bits + 1 bits
+static MsmPlan emul_plan(int c, int m, int scalar_bits) {
+  MsmPlan pl; pl.c = c; pl.W = (scalar_bits + c) / c; pl.nb = 1 << (c - 1); pl.m = m;
   // K = sum_w 2^(c-1) 2^(cw)
   uint32_t K[9] = {0};
   for (int w = 0; w < pl.W; w++) { int bit = c * w + c - 1; if (bit < 288) K[bit >> 5] |= 1u << (bit & 31); }
@@ -198,7 +199,7 @@ static int emul_msm_buckets(size_t n, const uint8_t* scalars, const uint8_t* pts
 template <class CV>
 static int emul_msm(size_t n, const uint8_t* scalars, const uint8_t* pts, int c, int m, uint8_t* out, int L = 0, int rounds = 0, int PB = 8, bool split = false) {
   using F = typename CV::F;
-  MsmPlan pl = emul_plan(c, m);
+  MsmPlan pl = emul_plan(c, m, CV::SCALAR_BITS);
   std::vector<Xyzz<F>> B;
   int rc = emul_msm_buckets<CV>(n, scalars, pts, pl, B, L, rounds, PB, split);
   if (rc) return rc;
@@ -219,7 +220,7 @@ template <class CV>
 static int emul_msm_exchange(size_t n, const uint8_t* scalars, const uint8_t* pts, int c, int m, int L, int rounds, int PB, int world, uint8_t* out, int m2 = 0) {
   using F = typename CV::F;
   using X = Xyzz<F>;
-  MsmPlan pl = emul_plan(c, m);
+  MsmPlan pl = emul_plan(c, m, CV::SCALAR_BITS);
   if (world < 1 || pl.W % world) return -2;
   const int wc = pl.W / world;
   std::vector<std::vector<X>> Bs(world);
@@ -375,5 +376,15 @@ int emul_bls12381_g2_decompress(const uint8_t* in96, uint8_t* out192) {
 void emul_bls12381_g2_mul_batch_w4(size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { emul_mul_batch_w4<Bls381G2>(n, s, p, o); }
 void emul_bls12381_g2_mul_batch(size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { emul_mul_batch<Bls381G2>(n, s, p, o); }
 int emul_bls12381_g2_msm(size_t n, const uint8_t* s, const uint8_t* p, int c, int m, int L, uint8_t* o) { return emul_msm<Bls381G2>(n, s, p, c, m, o, L); }
+}
+
+// ------------------------------------------------------------------------------------------------
+// the MSM template over the other groups: bn254 G2 (Fp2, 8 limbs), bn256 G1 (10 limbs) and bn256 G2 (Fp2, 10 limbs)
+#include "../../kyber_b200/csrc/bn_pairing.cuh"
+#include "../../kyber_b200/csrc/bn256.cuh"
+extern "C" {
+int emul_bn254_g2_msm(size_t n, const uint8_t* s, const uint8_t* p, int c, int m, int L, uint8_t* o) { return emul_msm<Bn254G2>(n, s, p, c, m, o, L); }
+int emul_bn256_g1_msm(size_t n, const uint8_t* s, const uint8_t* p, int c, int m, int L, uint8_t* o) { return emul_msm<Bn256G1>(n, s, p, c, m, o, L); }
+int emul_bn256_g2_msm(size_t n, const uint8_t* s, const uint8_t* p, int c, int m, int L, uint8_t* o) { return emul_msm<Bn256G2>(n, s, p, c, m, o, L); }
 }
 extern "C" void emul_set_pt_stage(int on) { g_pt_stage = on; }

@@ -392,3 +392,37 @@ def test_bn_hash_to_g1_bodies_against_reference_vectors():
         lib.emul_bn256_hash_to_g1(m, len(m), out64)
         assert out64.raw == o6.g1_marshal(o6.hash_to_g1(m))
 
+
+
+@pytest.mark.parametrize("group", ["bls12381_g1", "bls12381_g2", "bn254_g1", "bn254_g2", "bn256_g1", "bn256_g2"])
+def test_msm_bodies_every_group_and_input_set(emul, group):
+    """emul_msm (msm.cuh: digits, counting sort, slices or one thread per bucket, fix-up, chunk reduction, Horner) for each
+    group the device instantiates, on the input sets of tests/test_gpu_msm_curves.py (equal points in one bucket, P and -P,
+    infinities, empty upper windows, scalar edges, digit patterns that fill the largest bucket) through the forced (c, m, L)
+    shapes of its plans.  The operands repeat a few multipliers so that the oracle side stays cheap."""
+    import msm_cases as mc
+    g = mc.GROUPS[group]
+    fn = {"bls12381_g1": "emul_bls12381_g1_msm_v2", "bls12381_g2": "emul_bls12381_g2_msm", "bn254_g1": None,
+          "bn254_g2": "emul_bn254_g2_msm", "bn256_g1": "emul_bn256_g1_msm", "bn256_g2": "emul_bn256_g2_msm"}[group]
+    n = 96
+    A = mc.multipliers(g, 5)
+    operand = {0: bytes(g.in_bytes)}
+    for x in A + [g.r - A[0]]:
+        operand[x] = g.operand(g.mul(x))
+    assert operand[0] == g.operand(None)
+    for name in mc.SETS:
+        a, s = mc.build_set(g, name, n, A)
+        sb, pb = mc.scalars_to_bytes(s), b"".join(operand[x] for x in a)
+        want = g.expected(a, s)
+        for c, m, L in mc.EMUL_PLANS:
+            out = ctypes.create_string_buffer(g.out_bytes)
+            if fn is None:       # bn254 G1 enters through the affine-rounds wrapper with no rounds
+                rc = emul.emul_bn254_g1_msm_affine(ctypes.c_size_t(n), sb, pb, c, m, L, 0, 1, out)
+            else:
+                rc = getattr(emul, fn)(ctypes.c_size_t(n), sb, pb, c, m, L, out)
+            assert rc == 0 and out.raw == want, (group, name, c, m, L)
+    bad = mc.scalars_to_bytes([g.r] + s[1:])
+    out = ctypes.create_string_buffer(g.out_bytes)
+    rc = emul.emul_bn254_g1_msm_affine(ctypes.c_size_t(n), bad, pb, 4, 2, 3, 0, 1, out) if fn is None else \
+        getattr(emul, fn)(ctypes.c_size_t(n), bad, pb, 4, 2, 3, out)
+    assert rc == -3, group
