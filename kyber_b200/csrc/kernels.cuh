@@ -3,6 +3,7 @@
 #include "msm.cuh"
 #include "fp_inv.cuh"
 #include "msm_affine.cuh"
+#include "msm_sort.cuh"
 
 namespace b2k {
 
@@ -20,14 +21,34 @@ __global__ void __launch_bounds__(256) k_load_points(size_t n, const uint8_t* __
   pts[i] = p;
 }
 
-// ---- GLV front end (BLS12-381 G1): operand conversion + scalar split in one pass ------------------------------
-// pts[i] = +-P_i, pts[n+i] = +-(-phi(P_i)) = (beta x, -+y); vscalars[i], vscalars[n+i] = the two 127-bit magnitudes as
-// 32-byte big-endian scalars, so that the digit/sort stages run unchanged over 2n (scalar, point) pairs.
+// ---- MSM front end: digit columns + histogram from the pass that loads the points ------------------------------------------
+// Digit columns and histogram: msm_digits_store (msm_sort.cuh).
+//
+// groups without GLV: operand conversion, scalar range check and digits of pair i
+template <class CV>
+__global__ void __launch_bounds__(256) k_msm_load(size_t n, const uint8_t* __restrict__ scalars, const uint8_t* __restrict__ wire,
+                                                  Affine<typename CV::F>* __restrict__ pts, MsmPlan pl, int16_t* __restrict__ digits,
+                                                  uint32_t* __restrict__ counts, uint32_t* flags) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Affine<typename CV::F> p;
+  if (!load_checked<CV>(p, wire + (size_t)CV::IN_BYTES * i)) atomicOr(flags, FLAG_POINT);
+  pts[i] = p;
+  Scalar256 s;
+  scalar_load_be(s, scalars + 32 * i);
+  if (!scalar_in_range<typename CV::ScalarField>(s)) atomicOr(flags, FLAG_SCALAR_RANGE);
+  msm_digits_store(s, pl, n, i, digits, counts);
+}
+
+// ---- GLV front end (BLS12-381 G1): operand conversion + scalar split + digits in one pass -------------------------------------
+// pts[i] = +-P_i, pts[n+i] = +-(-phi(P_i)) = (beta x, -+y); the digits of the two 127-bit magnitudes go to rows i and n + i of the
+// digit columns (2n rows), so that the sort and accumulate stages run unchanged over 2n (scalar, point) pairs.
 // The launch covers pairs [i0, i0 + cnt) of the n of the call: the host-buffer MSM launches it once per chunk of its input copy.
 static __global__ void __launch_bounds__(256) k_glv_prepare_bls381(size_t n, size_t i0, size_t cnt, const uint8_t* __restrict__ scalars,
                                                                    const uint8_t* __restrict__ wire,
-                                                                   Affine<Fp<Bls381Fp>>* __restrict__ pts,
-                                                                   uint8_t* __restrict__ vscalars, uint32_t* flags) {
+                                                                   Affine<Fp<Bls381Fp>>* __restrict__ pts, MsmPlan pl,
+                                                                   int16_t* __restrict__ digits, uint32_t* __restrict__ counts,
+                                                                   uint32_t* flags) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= cnt) return;
   i += i0;
@@ -45,13 +66,8 @@ static __global__ void __launch_bounds__(256) k_glv_prepare_bls381(size_t n, siz
   glv_points_bls381(p, e, p0, sp);
   pts[i] = p;
   pts[n + i] = e;
-  uint32_t* o1 = reinterpret_cast<uint32_t*>(vscalars + 32 * i);          // big-endian bytes = byte-swapped words, top first
-  uint32_t* o2 = reinterpret_cast<uint32_t*>(vscalars + 32 * (n + i));
-#pragma unroll
-  for (int j = 0; j < 8; j++) {
-    o1[j] = __byte_perm(sp.k1.v[7 - j], 0, 0x0123);
-    o2[j] = __byte_perm(sp.k2.v[7 - j], 0, 0x0123);
-  }
+  msm_digits_store(sp.k1, pl, 2 * n, i, digits, counts);
+  msm_digits_store(sp.k2, pl, 2 * n, n + i, digits, counts);
 }
 
 // ---- independent scalar multiplications ----------------------------------------------------------
@@ -95,23 +111,6 @@ __global__ void __launch_bounds__(128, MINB) k_mul_batch(size_t n, const uint8_t
   jac_to_affine_bg(a, r);
   if (AFFINE_OUT) CV::store_affine(out + (size_t)CV::IN_BYTES * i, a);
   else CV::store(out + (size_t)CV::OUT_BYTES * i, a);
-}
-
-// ---- MSM stage 1: digits + histogram -------------------------------------------------------------
-template <class CV>
-__global__ void __launch_bounds__(256) k_msm_count(size_t n, const uint8_t* __restrict__ scalars, MsmPlan pl,
-                                                   uint32_t* __restrict__ counts, uint32_t* flags) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  Scalar256 s;
-  scalar_load_be(s, scalars + 32 * i);
-  if (!scalar_in_range<typename CV::ScalarField>(s)) atomicOr(flags, FLAG_SCALAR_RANGE);
-  uint32_t sp[9];
-  msm_recode(sp, s, pl.K);
-  for (int w = 0; w < pl.W; w++) {
-    int d = msm_digit(sp, pl.c, w);
-    if (d) atomicAdd(&counts[(size_t)w * pl.nb + (d < 0 ? -d : d) - 1], 1u);
-  }
 }
 
 // ---- MSM stage 2: exclusive scan of the histogram (3 small kernels, 1024 elements per block) -------
@@ -184,24 +183,7 @@ static __global__ void __launch_bounds__(1024) k_scan_finish(uint32_t total, con
   if (y == 0) cursor[i] = o;
 }
 
-// ---- MSM stage 3: counting-sort scatter ----------------------------------------------------------
-template <class CV>
-__global__ void __launch_bounds__(256) k_msm_scatter(size_t n, const uint8_t* __restrict__ scalars, MsmPlan pl,
-                                                     uint32_t* __restrict__ cursor, uint32_t* __restrict__ entries) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  Scalar256 s;
-  scalar_load_be(s, scalars + 32 * i);
-  uint32_t sp[9];
-  msm_recode(sp, s, pl.K);
-  for (int w = 0; w < pl.W; w++) {
-    int d = msm_digit(sp, pl.c, w);
-    if (d) {
-      uint32_t pos = atomicAdd(&cursor[(size_t)w * pl.nb + (d < 0 ? -d : d) - 1], 1u);
-      entries[pos] = (uint32_t)i | (d < 0 ? 0x80000000u : 0u);
-    }
-  }
-}
+// ---- MSM stage 3: bucket sort in two passes: k_msm_partition, k_msm_bin_sort (msm_sort.cuh) --------------------------------
 
 // ---- MSM stage 4: bucket accumulate (THE hot kernel) ---------------------------------------------
 template <class CV>

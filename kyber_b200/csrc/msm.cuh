@@ -8,9 +8,10 @@
 //
 // MSM pipeline (window c bits, W = ceil(256/c) windows, signed digits -> 2^(c-1) buckets/window):
 //   digits+count  : s' = s + K (K = sum of 2^(c-1) at every window) so that window digits of s' minus
-//                   2^(c-1) are the signed digits; histogram of (window, |digit|) by atomics
+//                   2^(c-1) are the signed digits; histogram of (window, |digit|) by atomics (in the pass that loads the
+//                   points, into window-major int16 digit columns: msm_sort.cuh)
 //   scan          : exclusive prefix sum of the histogram -> bucket start offsets
-//   scatter       : counting sort of (point index | sign) by bucket
+//   scatter       : counting sort of (point index | sign) by bucket, coarse partition + bin sort (msm_sort.cuh)
 //   accumulate    : one thread per bucket, XYZZ += +-P (mixed add 8M+2S), points gathered by index
 //   reduce        : per (window, chunk of m buckets): running sums  A = sum (k-k0) B_k,  S = sum B_k,
 //                   partial = A + k0*S ; then per-window tree sum of the partials

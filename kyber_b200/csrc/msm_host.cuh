@@ -203,8 +203,9 @@ size_t msm_scratch_bytes(const b2k_ctx* ctx, size_t n, const MsmPlan& pl) {
   size_t T = pl.nb / pl.m;
   size_t b = 0;
   b += pad256(n * sizeof(Affine<F>));
-  b += pad256(n * 32);                            // split scalars (GLV front end)
+  b += pad256(n * (size_t)pl.W * 2);              // digit columns (int16, window-major)
   b += pad256((total + 1) * 4) * 3;               // counts, offs, cursor
+  b += pad256(n * (size_t)pl.W * sizeof(SortRec)); // coarse-partitioned (entry, bucket) records of the bucket sort
   b += pad256(n * (size_t)pl.W * 4);              // entries
   b += pad256(total * sizeof(Xyzz<F>));           // buckets
   b += pad256((size_t)pl.W * T * sizeof(Xyzz<F>));  // partials
@@ -242,12 +243,11 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
   size_t total = (size_t)pl.W * pl.nb;
   int T = pl.nb / pl.m;
   auto* pts = arena_take<Affine<F>>(ctx, n);
-  uint8_t* vsc = glv ? arena_take<uint8_t>(ctx, n * 32) : nullptr;
-  const uint8_t* d_scalars = glv ? vsc : d_scalars_in;
-  if (glv && !vsc) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
+  auto* digits = arena_take<int16_t>(ctx, n * (size_t)pl.W);
   auto* counts = arena_take<uint32_t>(ctx, total + 1);
   auto* offs = arena_take<uint32_t>(ctx, total + 1);
   auto* cursor = arena_take<uint32_t>(ctx, total + 1);
+  auto* recs = arena_take<SortRec>(ctx, n * (size_t)pl.W);
   auto* entries = arena_take<uint32_t>(ctx, n * (size_t)pl.W);
   auto* own_buckets = arena_take<Xyzz<F>>(ctx, total);
   // bucket exchange (multi-GPU shape 1): the pipeline stops after the fix-up and leaves the W x 2^(c-1) buckets in the caller's buffer
@@ -260,7 +260,7 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
   const int S = window_sum_split(rp.TP);
   auto* wpart = arena_take<Xyzz<F>>(ctx, (size_t)pl.W * 128);
   if (!wpart) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
-  if (!pts || !counts || !offs || !cursor || !entries || !own_buckets || !partials || !runs || !wsum) {
+  if (!pts || !digits || !counts || !offs || !cursor || !recs || !entries || !own_buckets || !partials || !runs || !wsum) {
     ctx->err = "scratch arena too small";
     return B2K_ERR_ARG;
   }
@@ -272,7 +272,7 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
   auto* spart = arena_take<Xyzz<F>>(ctx, 2 * (size_t)(sa > smax ? sa : smax));
   auto* big_list = arena_take<uint32_t>(ctx, total + 1);
   auto* bsum = arena_take<uint32_t>(ctx, 1024 * (size_t)(1 + ap.R));   // block sums of the scan, 1024 words per column
-  if (!spart || !big_list || !bsum || total > 1024u * 1024u) {
+  if (!spart || !big_list || !bsum || total > 1024u * 1024u || (pl.nb >> sort_shift(pl.c)) > PART_BPW) {
     ctx->err = "scratch arena too small / too many buckets";
     return B2K_ERR_ARG;
   }
@@ -319,16 +319,15 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
         if (i0 >= n_in) break;
         const size_t cnt = (n_in - i0 < per) ? n_in - i0 : per;
         CK(cudaStreamWaitEvent(st, ctx->gev[1 + k], 0));
-        k_glv_prepare_bls381<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(n_in, i0, cnt, d_scalars_in, d_points, pts, vsc, ctx->d_flags);
+        k_glv_prepare_bls381<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(n_in, i0, cnt, d_scalars_in, d_points, pts, pl, digits, counts, ctx->d_flags);
       }
-    } else if (glv) k_glv_prepare_bls381<<<(unsigned)((n_in + 255) / 256), 256, 0, st>>>(n_in, 0, n_in, d_scalars_in, d_points, pts, vsc, ctx->d_flags);
-    else k_load_points<CV><<<gb_n, 256, 0, st>>>(n, d_points, pts, ctx->d_flags);
+    } else if (glv) k_glv_prepare_bls381<<<(unsigned)((n_in + 255) / 256), 256, 0, st>>>(n_in, 0, n_in, d_scalars_in, d_points, pts, pl, digits, counts, ctx->d_flags);
+    else k_msm_load<CV><<<gb_n, 256, 0, st>>>(n, d_scalars_in, d_points, pts, pl, digits, counts, ctx->d_flags);
   } else {
-    k_load_points<CV><<<gb_n, 256, 0, st>>>(n, d_points, pts, ctx->d_flags);
+    k_msm_load<CV><<<gb_n, 256, 0, st>>>(n, d_scalars_in, d_points, pts, pl, digits, counts, ctx->d_flags);
   }
   nl++;
-  CK(cudaEventRecord(ctx->ev[1], st));
-  k_msm_count<CV><<<gb_n, 256, 0, st>>>(n, d_scalars, pl, counts, ctx->d_flags); nl++;
+  CK(cudaEventRecord(ctx->ev[1], st));             // the digits and the histogram come out of the load pass: ev[1..2] is empty
   CK(cudaEventRecord(ctx->ev[2], st));
   {
     const dim3 cols(sblocks, 1 + ap.R), tops(1, 1 + ap.R);     // the histogram + the bucket sizes after each affine round
@@ -337,7 +336,13 @@ int msm_enqueue(b2k_ctx* ctx, size_t n_in, const MsmPlan& pl, const uint8_t* d_s
     k_scan_finish<<<cols, 1024, 0, st>>>((uint32_t)total, bsum, offs, offs_rt, cursor); nl += 3;
   }
   CK(cudaEventRecord(ctx->ev[3], st));
-  k_msm_scatter<CV><<<gb_n, 256, 0, st>>>(n, d_scalars, pl, cursor, entries); nl++;
+  {
+    const int S = sort_shift(pl.c);
+    const size_t nrec = n * (size_t)pl.W;
+    k_msm_partition<<<(unsigned)((n + PART_TILE - 1) / PART_TILE), PART_T, 0, st>>>((uint32_t)n, pl, S, digits, cursor, recs);
+    k_msm_bin_sort<<<(unsigned)((nrec + BSORT_TILE - 1) / BSORT_TILE), BSORT_T, 0, st>>>((uint32_t)total, S, recs, offs, counts, entries);
+    nl += 2;
+  }
   const int G = (!ext_buckets && !ctx->use_v1 && ctx->msm_groups > 1 && pl.W >= 2 * ctx->msm_groups && ctx->stream2) ? ctx->msm_groups : 1;
   if (G > 1) {
     // ---- overlapped tail: groups of windows, top group first; reduction of group g on stream2 while the main

@@ -1,11 +1,13 @@
 """Per-kernel time of one BLS12-381 G1 MSM over 2^20 distinct pairs resident on the device (the shape bench.py measures),
 taken with torch.profiler (CUDA activities) in a run of its own.  Usage:
 
-    python tools/perf_kernels.py OUTDIR [--rounds R] [--batch B] [--split 0|1] [--msms K]
+    python tools/perf_kernels.py OUTDIR [--rounds R] [--batch B] [--split 0|1] [--msms K] [--set uniform|equal|bdn128]
 
 The MSM is warmed up outside the profiler, then K MSMs (default 1) run back to back on one stream under it.  Written to OUTDIR:
 kernels.txt (table: kernel, launches per MSM, total / mean microseconds per MSM, share of the MSM's device span) and kernels.json
-(the same rows plus the GPU's name, power limit and the plan the MSMs ran with).  Every MSM's output is checked against the oracle."""
+(the same rows plus the GPU's name, power limit and the plan the MSMs ran with).  Every MSM's output is checked against the oracle.
+--set picks the input: uniform scalars and distinct points (default), one (s, P) repeated 2^20 times (every window's entries in one
+bucket), or 128-bit BDN-style factors (s mod 2^128 + 1) over the distinct points."""
 import argparse
 import json
 import os
@@ -48,6 +50,7 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="outputs per thread of a round (0 = automatic)")
     ap.add_argument("--split", type=int, default=1, help="1 = split round kernels (library default), 0 = fused")
     ap.add_argument("--msms", type=int, default=1, help="MSMs inside the profiled region")
+    ap.add_argument("--set", default="uniform", choices=("uniform", "equal", "bdn128"), help="input set (skewed scalars: equal, bdn128)")
     args = ap.parse_args()
 
     import torch
@@ -62,6 +65,10 @@ def main():
     eng.set_msm_affine(args.rounds, args.batch)
     a = wl.prng_scalars("b2k/c2-a", n, o.R)
     s = wl.prng_scalars("b2k/c2", n, o.R)
+    if args.set == "equal":
+        a, s = [a[0]] * n, [s[0]] * n
+    elif args.set == "bdn128":
+        s = [x % (1 << 128) + 1 for x in s]
     base = eng.bls12381_g1_mul_batch_affine(wl.scalars_to_bytes(a), wl.G1_BLS12381_AFFINE * n)
     want = o.g1_compress(o.g1_mul(wl.dot_mod(s, a, o.R)))
     pts = torch.frombuffer(bytearray(base), dtype=torch.uint8).cuda()
@@ -101,14 +108,14 @@ def main():
     plan = eng.last_msm_plan()
     os.makedirs(args.outdir, exist_ok=True)
     with open(os.path.join(args.outdir, "kernels.txt"), "w") as f:
-        f.write(f"# BLS12-381 G1 MSM, 2^20 pairs, one stream, {K} MSM(s) under torch.profiler (CUDA activities); per MSM\n")
+        f.write(f"# BLS12-381 G1 MSM, 2^20 pairs ({args.set} set), one stream, {K} MSM(s) under torch.profiler (CUDA activities); per MSM\n")
         f.write(f"# GPU: {gname}, power limit {plim}; plan: {json.dumps(plan)}\n")
         f.write(f"# device span {span / 1e3:.3f} ms per MSM, kernels + memsets busy {busy / 1e3:.3f} ms, {launches:.0f} library launches\n")
         f.write(f"{'kernel':72s} {'count':>6s} {'total_us':>10s} {'mean_us':>9s} {'share':>6s}\n")
         for k, c, t, m, sh in table:
             f.write(f"{k[:72]:72s} {c:6.1f} {t:10.1f} {m:9.1f} {100 * sh:5.1f}%\n")
     with open(os.path.join(args.outdir, "kernels.json"), "w") as f:
-        json.dump({"gpu": gname, "power_limit": plim, "msms": K, "span_us_per_msm": span, "busy_us_per_msm": busy,
+        json.dump({"set": args.set, "gpu": gname, "power_limit": plim, "msms": K, "span_us_per_msm": span, "busy_us_per_msm": busy,
                    "launches_per_msm": launches, "plan": plan,
                    "kernels": [{"name": k, "count": c, "total_us": t, "mean_us": m, "share": sh} for k, c, t, m, sh in table]}, f, indent=1)
     print(open(os.path.join(args.outdir, "kernels.txt")).read())
