@@ -451,6 +451,27 @@ int b2k_ed25519_mul_batch(b2k_ctx* ctx, size_t n, const uint8_t* scalars /*[n][3
                           const uint8_t* points /*[n][32]*/, uint8_t* out /*[n][32]*/);
 int b2k_ed25519_mul_batch_dev(b2k_ctx* ctx, size_t n, const void* d_scalars, const void* d_points, void* d_out);
 
+/* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
+ * the FIRST check that fails, in the reference's order:
+ *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical
+ *   2 R's y >= p (point.IsCanonical)           -> ErrPointRNotCanonical
+ *   3 R does not decode                        -> ErrPointRInvalid
+ *   4 R has order 1, 2, 4 or 8 (HasSmallOrder) -> ErrPointRSmallOrder
+ *   5, 6, 7 the same three checks on the key   -> ErrPKNotCanonical, ErrPKInvalid, ErrPKSmallOrder
+ *   8 encode(s B) != encode(R + h A), h = SHA-512(R || pk || msg) mod l, cofactorless -> ErrSignatureRecNotEqual
+ * Signatures (R || s) and keys have a fixed stride, so the reference's length errors are the caller's checks;
+ * ErrSchnorrInvalidScalar cannot occur for 32 bytes.  msgs/offsets as in b2k_bls12381_verify_g1sig (decreasing offsets ->
+ * B2K_ERR_ARG from the host form).  Bad data is never a call error, only a status.  The host form stages every input in
+ * one device allocation and synchronises; the _dev form takes device pointers and only enqueues.
+ * replaces: eddsa.Verify / VerifyWithChecks called in a loop (e.g. sign/dss/dss.go:216). */
+enum { B2K_ED_OK = 0, B2K_ED_SIG_NOT_CANONICAL = 1, B2K_ED_R_NOT_CANONICAL = 2, B2K_ED_R_INVALID = 3,
+       B2K_ED_R_SMALL_ORDER = 4, B2K_ED_PK_NOT_CANONICAL = 5, B2K_ED_PK_INVALID = 6, B2K_ED_PK_SMALL_ORDER = 7,
+       B2K_ED_NOT_EQUAL = 8 };
+int b2k_ed25519_verify(b2k_ctx* ctx, size_t n, const uint8_t* pks /*[n][32]*/, const uint8_t* msgs,
+                       const uint32_t* offsets /*[n+1]*/, const uint8_t* sigs /*[n][64] R||s*/, uint8_t* status /*[n]*/);
+int b2k_ed25519_verify_dev(b2k_ctx* ctx, size_t n, const void* d_pks, const void* d_msgs, const void* d_offsets,
+                           const void* d_sigs, void* d_status);
+
 /* ---- hash-to-G1 on the BN curves ------------------------------------------------------------------------- */
 /* out[i] = Hash(msg_i) as 64 bytes x||y; msgs/offsets as in b2k_bls12381_hash_to_g1 (offsets[n+1], msg_i =
  * msgs[offsets[i] .. offsets[i+1])).

@@ -65,6 +65,8 @@ def load_library() -> C.CDLL:
     sigs["b2k_bls12381_verify_g2sig_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, C.c_uint32, vp, vp])
     sigs["b2k_bls12381_verify_g1sig"] = (C.c_int, [vp, sz, vp, vp, vp, vp, C.c_uint32, vp, vp])
     sigs["b2k_bls12381_verify_g1sig_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, C.c_uint32, vp, vp])
+    sigs["b2k_ed25519_verify"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_verify_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -502,6 +504,22 @@ class Engine:
         n = len(scalars_le) // 32
         assert len(scalars_le) == 32 * n and len(points) == 32 * n
         return self.call_host("b2k_ed25519_mul_batch", n, scalars_le, points, 32 * n)
+
+    def ed25519_verify(self, pks: bytes, msgs, sigs: bytes) -> bytes:
+        """n x eddsa.VerifyWithChecks: pks [n][32], msgs list of bytes, sigs [n][64] R || s -> one status byte each
+        (0 = valid, else the first failing check, B2K_ED_* of include/b2kyber.h)"""
+        n = len(msgs)
+        assert len(pks) == 32 * n and len(sigs) == 64 * n
+        blob, offs = self._pack_msgs(msgs)
+        status = bytearray(n)
+        bufs = [_buf(x) for x in (pks, blob, offs, sigs, status)]
+        self._check(self.lib.b2k_ed25519_verify(self.h, n, *[b[0] for b in bufs]))
+        return bytes(status)
+
+    def ed25519_verify_dev(self, n: int, d_pks: int, d_msgs: int, d_offsets: int, d_sigs: int, d_status: int):
+        """the same on device pointers ([n][32], message bytes, [n+1] uint32 offsets, [n][64], [n] status); enqueue only"""
+        self._check(self.lib.b2k_ed25519_verify_dev(self.h, n, C.c_void_p(d_pks), C.c_void_p(d_msgs), C.c_void_p(d_offsets),
+                                                    C.c_void_p(d_sigs), C.c_void_p(d_status)))
 
     def bn254_pair(self, g1: bytes, g2: bytes) -> bytes:
         n = len(g1) // 64

@@ -73,13 +73,6 @@ __global__ void __launch_bounds__(64) k_g2_decompress_v(size_t n, const uint8_t*
 
 }  // namespace b2k
 
-// message offsets of the host entry points: non-decreasing (ADVICE r1: a decreasing pair would make a kernel read ~4 GiB)
-static int check_offsets(b2k_ctx* ctx, size_t n, const uint32_t* offsets) {
-  for (size_t i = 0; i < n; i++)
-    if (offsets[i + 1] < offsets[i]) { ctx->err = "message offsets must be non-decreasing"; return B2K_ERR_ARG; }
-  return B2K_OK;
-}
-
 extern "C" {
 
 int b2k_bls12381_hash_to_g1_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, const void* d_offsets, const void* d_dst,

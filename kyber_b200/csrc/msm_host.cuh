@@ -111,6 +111,13 @@ inline int check_flags(b2k_ctx* ctx) {
   return B2K_OK;
 }
 
+// message offsets of the host entry points: non-decreasing (ADVICE r1: a decreasing pair would make a kernel read ~4 GiB)
+inline int check_offsets(b2k_ctx* ctx, size_t n, const uint32_t* offsets) {
+  for (size_t i = 0; i < n; i++)
+    if (offsets[i + 1] < offsets[i]) { ctx->err = "message offsets must be non-decreasing"; return B2K_ERR_ARG; }
+  return B2K_OK;
+}
+
 // host-buffer entry points: the device status word is cleared in front of the call's work, fetched AND cleared behind it
 // (a failed call must not leave a stale bit for a later *_dev sequence + b2k_wait)
 inline int status_begin(b2k_ctx* ctx) {

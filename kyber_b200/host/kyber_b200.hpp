@@ -442,6 +442,25 @@ class Curve {
     return out;
   }
   PointBytes Mul(const PointBytes& s, const PointBytes* A) const { return MulBatch({s}, {A ? *A : BASE})[0]; }   // nil = base point
+  // status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msgs[i], sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the
+  // B2K_ED_* code of the first check that fails.  Signatures are R || s; a signature of another length is the caller's
+  // ErrSignatureLength.
+  std::vector<uint8_t> VerifyBatch(const std::vector<PointBytes>& pks, const std::vector<std::vector<uint8_t>>& msgs,
+                                   const std::vector<std::array<uint8_t, 64>>& sigs) const {
+    size_t n = pks.size();
+    if (msgs.size() != n || sigs.size() != n) throw std::logic_error("VerifyBatch: length mismatch");
+    std::vector<uint8_t> status(n);
+    if (n == 0) return status;
+    std::vector<uint32_t> offs(n + 1, 0);
+    std::vector<uint8_t> blob;
+    for (size_t i = 0; i < n; i++) {
+      blob.insert(blob.end(), msgs[i].begin(), msgs[i].end());
+      offs[i + 1] = (uint32_t)blob.size();
+    }
+    if (blob.empty()) blob.push_back(0);
+    eng_->check(b2k_ed25519_verify(eng_->ctx(), n, pks[0].data(), blob.data(), offs.data(), sigs[0].data(), status.data()));
+    return status;
+  }
  private:
   std::shared_ptr<Engine> eng_;
 };
