@@ -148,7 +148,7 @@ int b2k_last_timings(b2k_ctx* ctx, float* ms, int max) {
 
 int b2k_last_msm_plan(const b2k_ctx* ctx, int* out, int max) {
   if (!ctx || !out || max <= 0) return B2K_ERR_ARG;
-  int n = max < 20 ? max : 20;
+  int n = max < LP_SLOTS ? max : LP_SLOTS;
   for (int i = 0; i < n; i++) out[i] = ctx->last_plan[i];
   return n;
 }
@@ -253,9 +253,9 @@ int b2k_set_msm_layout(b2k_ctx* ctx, int layout) {
 int b2k_bls12381_g1_msm_affine_dev(b2k_ctx* c, size_t n, const void* s, const void* p, void* o) { return msm_dev<Bls381G1>(c, n, s, p, o, 1); }
 
 int b2k_bls12381_g1_msm_bucket_plan(b2k_ctx* c, size_t n, int* plan) { return msm_bucket_plan<Bls381G1>(c, n, plan); }
-int b2k_bls12381_g1_msm_buckets_dev(b2k_ctx* c, size_t n, const void* s, const void* p, void* b, size_t cap, int* plan) { return msm_buckets_dev<Bls381G1>(c, n, s, p, b, cap, plan); }
+int b2k_bls12381_g1_msm_buckets_dev(b2k_ctx* c, size_t n, const void* s, const void* p, void* b, size_t cap, int* plan) { return msm_buckets<Bls381G1>(c, n, (const uint8_t*)s, (const uint8_t*)p, false, b, cap, plan); }
 // internal (b2k_ctx.h): host-staged bucket pass for the sharded entry points of b2k_multi.cu
-int b2k_internal_bls12381_g1_msm_buckets_host(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, void* b, size_t cap, int* plan) { return msm_buckets_host<Bls381G1>(c, n, s, p, b, cap, plan); }
+int b2k_internal_bls12381_g1_msm_buckets_host(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, void* b, size_t cap, int* plan) { return msm_buckets<Bls381G1>(c, n, s, p, true, b, cap, plan); }
 int b2k_bls12381_g1_msm_reduce_windows_dev(b2k_ctx* c, int cbits, int w_cnt, int parts, const void* recv, void* wsum) { return msm_reduce_windows_dev<Bls381G1>(c, cbits, w_cnt, parts, recv, wsum); }
 int b2k_bls12381_g1_msm_finish_dev(b2k_ctx* c, int cbits, int W, const void* wsum, void* out, int affine_out) { return msm_finish_dev<Bls381G1>(c, cbits, W, wsum, out, affine_out); }
 

@@ -6,6 +6,18 @@
 
 constexpr int B2K_N_EV = 12;
 
+// slots of b2k_ctx::last_plan, the layout b2k_last_msm_plan returns (kyber_b200/capi.py: last_msm_plan decodes it)
+enum MsmPlanSlot {
+  LP_C = 0, LP_W, LP_NB, LP_M,   // window bits, windows, buckets per window, single-level chunk
+  LP_SLICE,                      // slice length the XYZZ slices ran with
+  LP_ROUNDS,                     // affine rounds
+  LP_BATCH,                      // their batch widths, one slot per possible round (8)
+  LP_GLV = LP_BATCH + 8,
+  LP_SPLIT,                      // affine rounds as three kernels
+  LP_LEVELS, LP_M1, LP_M2,       // bucket reduction: levels and chunk per level (LP_M2 = 0 for one level)
+  LP_SLOTS = 20
+};
+
 struct b2k_arena {
   char* base = nullptr;
   size_t cap = 0, used = 0;
@@ -50,7 +62,7 @@ struct b2k_ctx {
   void* pair_scratch = nullptr;     // Miller values between the two kernels of the split pairing (576 B per element; grown on demand)
   size_t pair_scratch_cap = 0;
   int msm_layout = 0;   // 0 = compact field products (library default), 1 = inlined at every use (b2k_msm_inlined.cu): A/B aid
-  int last_plan[20] = {};           // what the last MSM ran with: c, W, buckets/window, chunk, slice length, affine rounds, their batch widths
+  int last_plan[LP_SLOTS] = {};     // what the last MSM ran with (MsmPlanSlot)
   uint64_t launches = 0;
   std::string err;
 };

@@ -209,48 +209,27 @@ PeerPtrs peer_ptrs(const b2k_comm* cm) {
   } while (0)
 
 // windows of this rank reduced from `parts` sources into cm's slab region wsum[w_lo .. w_lo + w_cnt)
-int reduce_owned_windows(b2k_comm* cm, int c, int W, int w_lo, int w_cnt, bool from_peers) {
+int reduce_owned_windows(b2k_comm* cm, int c, int w_lo, int w_cnt, bool from_peers) {
   b2k_ctx* ctx = cm->ctx;
   cudaStream_t st = ctx->stream;
   const int nb = 1 << (c - 1);
-  int m = 1;
-  while (m < 64 && m * 2 <= nb && ((size_t)w_cnt * nb) / (size_t)(m * 2) >= 16384) m *= 2;
-  if (ctx->force_m > 0 && ctx->force_m <= nb && (ctx->force_m & (ctx->force_m - 1)) == 0) m = ctx->force_m;
-  const ReducePlan rp = reduce_plan(ctx, nb, m);
-  const int S = window_sum_split(rp.TP);
-  int rc = arena_reserve(ctx, pad256((size_t)w_cnt * rp.TP * sizeof(X)) + pad256((size_t)w_cnt * rp.T1 * sizeof(X)) +
-                                  pad256((size_t)w_cnt * 128 * sizeof(X)) + pad256((size_t)w_cnt * sizeof(X)) + 4096);
+  const ReducePlan rp = owned_reduce_plan(ctx, nb, w_cnt);
+  TailBufs<X> t;
+  X* mine = nullptr;
+  int rc = arena_carve(ctx, [&](Carve& cv) {
+    t.carve(cv, w_cnt, rp.TP, rp);
+    mine = cv.take<X>(w_cnt);
+  });
   if (rc) return rc;
-  auto* partials = arena_take<X>(ctx, (size_t)w_cnt * rp.TP);
-  auto* runs = arena_take<X>(ctx, (size_t)w_cnt * rp.T1);
-  auto* wpart = arena_take<X>(ctx, (size_t)w_cnt * 128);
-  auto* mine = arena_take<X>(ctx, (size_t)w_cnt);
-  if (!partials || !runs || !wpart || !mine) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
-  const size_t n1 = (size_t)w_cnt * rp.T1;
-  if (from_peers) {
-    k_msm_reduce_l1_peers<<<(unsigned)((n1 + 127) / 128), 128, 0, st>>>(nb, rp.m1, rp.m2, rp.levels, w_lo, w_cnt, cm->nranks, cm->rank,
-                                                                         peer_ptrs(cm), partials, runs);
-  } else {                                     // NCCL transport: recv = [parts][w_cnt][nb]
-    const X* recv = reinterpret_cast<const X*>(cm->recv);
-    if (rp.levels == 2) k_msm_reduce_l1<CV><<<(unsigned)((n1 + 127) / 128), 128, 0, st>>>(nb, rp.m1, rp.m2, w_cnt, cm->nranks, recv, partials, runs);
-    else k_msm_reduce_chunks_parts<CV><<<(unsigned)((n1 + 127) / 128), 128, 0, st>>>(nb, rp.m1, w_cnt, cm->nranks, recv, partials);
-  }
-  ctx->launches += 1;
-  if (rp.levels == 2) {
-    const size_t n2 = (size_t)w_cnt * (rp.T1 / rp.m2);
-    k_msm_reduce_l2<CV><<<(unsigned)((n2 + 127) / 128), 128, 0, st>>>(nb, rp.m1, rp.m2, rp.log2_m1, w_cnt, runs, partials);
-    ctx->launches += 1;
-  }
-  if (S > 1) {
-    k_msm_window_sum<CV><<<w_cnt * S, 128, 0, st>>>(rp.TP / S, partials, wpart);
-    k_msm_window_sum<CV><<<w_cnt, 128, 0, st>>>(S, wpart, mine);
-    ctx->launches += 2;
-  } else {
-    k_msm_window_sum<CV><<<w_cnt, 128, 0, st>>>(rp.TP, partials, mine);
-    ctx->launches += 1;
-  }
+  const X* recv = reinterpret_cast<const X*>(cm->recv);   // NCCL transport: recv = [parts][w_cnt][nb]
+  rc = reduce_windows<CV>(ctx, nb, w_cnt, rp, t, mine, [&](unsigned grid) {
+    if (from_peers)
+      k_msm_reduce_l1_peers<<<grid, 128, 0, st>>>(nb, rp.m1, rp.m2, rp.levels, w_lo, w_cnt, cm->nranks, cm->rank, peer_ptrs(cm), t.partials, t.runs);
+    else if (rp.levels == 2) k_msm_reduce_l1<CV><<<grid, 128, 0, st>>>(nb, rp.m1, rp.m2, w_cnt, cm->nranks, recv, t.partials, t.runs);
+    else k_msm_reduce_chunks_parts<CV><<<grid, 128, 0, st>>>(nb, rp.m1, w_cnt, cm->nranks, recv, t.partials);
+  });
+  if (rc) return rc;
   CK(cudaGetLastError());
-  (void)W;
   // the window sums of this rank go to every rank (own slab included)
   if (cm->nccl) {
     CKN(g_nccl.AllGather(mine, cm->slab + OFF_WSUM, (size_t)w_cnt * sizeof(X), NCCL_UINT8, cm->nccl, st));
@@ -278,13 +257,13 @@ int exchange_and_finish(b2k_comm* cm, const int* plan, void* d_out) {
       CKN(g_nccl.Recv(cm->recv + (size_t)p * chunk, chunk, NCCL_UINT8, p, cm->nccl, st));
     }
     CKN(g_nccl.GroupEnd());
-    int rc = reduce_owned_windows(cm, c, W, w_lo, w_cnt, false);
+    int rc = reduce_owned_windows(cm, c, w_lo, w_cnt, false);
     if (rc) return rc;
   } else {
     k_comm_signal<<<1, 32, 0, st>>>(peer_ptrs(cm), cm->nranks, cm->rank, F_READY, cm->step);
     k_comm_wait<<<1, 32, 0, st>>>(cm->slab, cm->nranks, F_READY, cm->step, ctx->d_flags);
     ctx->launches += 2;
-    int rc = reduce_owned_windows(cm, c, W, w_lo, w_cnt, true);
+    int rc = reduce_owned_windows(cm, c, w_lo, w_cnt, true);
     if (rc) return rc;
     // the peers may overwrite their buckets once every reader is done: publish "done reading step s" (k_comm_push already
     // follows the reduction kernels in stream order, a separate flag keeps the two meanings apart)

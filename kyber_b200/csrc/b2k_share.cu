@@ -128,23 +128,23 @@ __global__ void __launch_bounds__(128) k_pubpoly_check(uint32_t m, uint32_t t, c
 
 template <class CV, class FR>
 static int recover_commit(b2k_ctx* ctx, size_t t, const uint32_t* indices, const uint8_t* points, uint8_t* out) {
-  if (!ctx || !indices || !points || !out || t == 0 || t >= (size_t(1) << 31)) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  MsmPlan pl = msm_plan<CV>(ctx, t);
-  size_t extra = pad256(t * 4) + pad256(t * 32) + pad256(t * (size_t)CV::IN_BYTES) + 1024;
-  int rc = arena_reserve(ctx, msm_scratch_bytes<CV>(ctx, msm_virtual_n<CV>(ctx, t), pl) + extra);
+  MsmLayout<CV> s;
+  uint32_t* d_idx = nullptr;
+  uint8_t *d_s = nullptr, *d_p = nullptr, *d_o = nullptr;
+  int rc = msm_begin<CV>(ctx, t, indices && points && out, s, [&](Carve& c) {
+    d_idx = c.take<uint32_t>(t);
+    d_s = c.take<uint8_t>(t * 32);
+    d_p = c.take<uint8_t>(t * (size_t)CV::IN_BYTES);
+    d_o = c.take<uint8_t>(256);
+  });
   if (rc) return rc;
-  uint32_t* d_idx = arena_take<uint32_t>(ctx, t);
-  uint8_t* d_s = arena_take<uint8_t>(ctx, t * 32);
-  uint8_t* d_p = arena_take<uint8_t>(ctx, t * (size_t)CV::IN_BYTES);
-  uint8_t* d_o = arena_take<uint8_t>(ctx, 256);
   cudaStream_t st = ctx->stream;
   CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
   CK(cudaMemcpyAsync(d_idx, indices, t * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_p, points, t * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, st));
   k_lagrange_at_zero<FR><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, d_idx, d_s, ctx->d_flags);
   ctx->launches += 1;
-  rc = msm_enqueue<CV>(ctx, t, pl, d_s, d_p, d_o);
+  rc = msm_enqueue<CV>(ctx, s, d_s, d_p, d_o);
   if (rc) return rc;
   CK(cudaMemcpyAsync(out, d_o, CV::OUT_BYTES, cudaMemcpyDeviceToHost, st));
   rc = status_fetch_async(ctx);
