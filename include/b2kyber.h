@@ -451,6 +451,35 @@ int b2k_ed25519_mul_batch(b2k_ctx* ctx, size_t n, const uint8_t* scalars /*[n][3
                           const uint8_t* points /*[n][32]*/, uint8_t* out /*[n][32]*/);
 int b2k_ed25519_mul_batch_dev(b2k_ctx* ctx, size_t n, const void* d_scalars, const void* d_points, void* d_out);
 
+/* ---- edwards25519 MSM and share/poly -------------------------------------------------------------------------------------
+ * Points: 32-byte compressed, decoded like FromBytes (ge.go:110-150, non-canonical y accepted); a point that does not decode
+ * -> B2K_ERR_POINT and its term counts as the identity.  Results: the canonical ToBytes encoding.  The identity is 01 00..00;
+ * all-zero bytes decode to a point of order 4, NOT to the identity.
+ * Scalars: 32-byte little-endian, read as the reference's Point.Mul reads them (geScalarMult, ge.go:443-502): the plain integer
+ * (no reduction mod l, so torsion parts of the points count), except when the top digit e63 = (k >> 252) + carry of its
+ * signed-nibble recoding exceeds 8: selectCached (ge.go:419-433) then selects nothing and the term is (k - e63 2^252) P.
+ * Indices: x = index + 1 (index 0xffffffff gives 2^32), as in the other groups' share entry points.
+ * b2k_last_msm_plan [0..4] and b2k_last_timings report the last MSM / RecoverCommit ([0] includes the point decoding). */
+/* out = sum_i scalars[i] * points[i].  replaces: the Point.Mul + Add loops over edwards25519 (share/poly.go:461-473,
+ * sign/cosi's aggregate of commitments), one call instead of n Mul. */
+int b2k_ed25519_msm(b2k_ctx* ctx, size_t n, const uint8_t* scalars /*[n][32] LE*/, const uint8_t* points /*[n][32]*/,
+                    uint8_t* out /*[32]*/);
+/* device pointers; enqueue only: data errors (B2K_ERR_POINT) arrive at b2k_wait */
+int b2k_ed25519_msm_dev(b2k_ctx* ctx, size_t n, const void* d_scalars, const void* d_points, void* d_out);
+/* out = sum_i lambda_i points[i], lambda_i = prod_{j != i} x_j / (x_j - x_i) mod l: share.RecoverCommit (share/poly.go:449-476,
+ * also pvss.RecoverSecret pvss.go:322 and DKG resharing dkg.go:965) after xyCommit's selection.  Duplicate indices -> B2K_ERR_ARG. */
+int b2k_ed25519_recover_commit(b2k_ctx* ctx, size_t t, const uint32_t* indices /*[t]*/, const uint8_t* points /*[t][32]*/,
+                               uint8_t* out /*[32]*/);
+/* out[i] = sum_j (indices[i] + 1)^j commits[j] (Horner): share.PubPoly.Eval (share/poly.go:340-357) for n indices. */
+int b2k_ed25519_pubpoly_eval(b2k_ctx* ctx, size_t t, const uint8_t* commits /*[t][32]*/, size_t n, const uint32_t* indices /*[n]*/,
+                             uint8_t* out /*[n][32]*/);
+/* ok[d][k] = ( sum_j (indices[d][k] + 1)^j commits[d][j] == shares[d][k] * B ), B the base point, one byte per check:
+ * share.PubPoly.Check (share/poly.go:405-409) as run once per deal, response and justification in
+ * share/vss/pedersen/vss.go:636-645 and share/dkg/pedersen/dkg.go:489-494, 826-834.  shares: 32-byte little-endian, read
+ * like the scalars above (Check's Mul(s.V, p.b) goes through geScalarMult). */
+int b2k_ed25519_pubpoly_check(b2k_ctx* ctx, size_t m, size_t t, const uint8_t* commits /*[m][t][32]*/, size_t n,
+                              const uint32_t* indices /*[m][n]*/, const uint8_t* shares /*[m][n][32] LE*/, uint8_t* ok /*[m][n]*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

@@ -67,6 +67,9 @@ def load_library() -> C.CDLL:
     sigs["b2k_bls12381_verify_g1sig_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, C.c_uint32, vp, vp])
     sigs["b2k_ed25519_verify"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_ed25519_verify_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
+    sigs["b2k_ed25519_pubpoly_eval"] = (C.c_int, [vp, sz, vp, sz, vp, vp])
+    sigs["b2k_ed25519_pubpoly_check"] = (C.c_int, [vp, sz, sz, vp, sz, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -125,13 +128,13 @@ HOST_FUNCS = [
     "b2k_bls12381_g2_mul_batch", "b2k_bls12381_g2_mul_batch_affine", "b2k_bls12381_g2_msm",
     "b2k_bls12381_g1_decompress", "b2k_bls12381_g2_decompress",
     "b2k_bls12381_g1_mul_batch", "b2k_bls12381_g1_mul_batch_affine", "b2k_bls12381_g1_msm",
-    "b2k_bn254_g1_mul_batch", "b2k_bn254_g1_msm", "b2k_ed25519_mul_batch",
+    "b2k_bn254_g1_mul_batch", "b2k_bn254_g1_msm", "b2k_ed25519_mul_batch", "b2k_ed25519_msm",
 ]
 DEV_FUNCS = [
     "b2k_bls12381_g2_mul_batch_affine_dev", "b2k_bls12381_g2_msm_dev",
     "b2k_bls12381_g1_decompress_dev", "b2k_bls12381_g2_decompress_dev",
     "b2k_bls12381_g1_mul_batch_dev", "b2k_bls12381_g1_mul_batch_affine_dev", "b2k_bls12381_g1_msm_dev",
-    "b2k_bls12381_g1_msm_affine_dev", "b2k_bn254_g1_msm_dev", "b2k_ed25519_mul_batch_dev",
+    "b2k_bls12381_g1_msm_affine_dev", "b2k_bn254_g1_msm_dev", "b2k_ed25519_mul_batch_dev", "b2k_ed25519_msm_dev",
 ]
 
 
@@ -504,6 +507,46 @@ class Engine:
         n = len(scalars_le) // 32
         assert len(scalars_le) == 32 * n and len(points) == 32 * n
         return self.call_host("b2k_ed25519_mul_batch", n, scalars_le, points, 32 * n)
+
+    def ed25519_msm(self, scalars_le: bytes, points: bytes) -> bytes:
+        """sum_i k_i P_i on edwards25519: little-endian 32-byte scalars read as Point.Mul reads them, 32-byte compressed
+        points -> the 32-byte encoding of the sum"""
+        n = len(scalars_le) // 32
+        assert len(scalars_le) == 32 * n and len(points) == 32 * n
+        return self.call_host("b2k_ed25519_msm", n, scalars_le, points, 32)
+
+    def ed25519_msm_dev(self, n: int, d_scalars: int, d_points: int, d_out: int):
+        """the same on device pointers ([n][32], [n][32], [32]); enqueue only, data errors at wait()"""
+        self.call_dev("b2k_ed25519_msm_dev", n, d_scalars, d_points, d_out)
+
+    def ed25519_recover_commit(self, indices, points: bytes) -> bytes:
+        """share.RecoverCommit over edwards25519: share indices I_i (x_i = I_i + 1), points [t][32] -> 32 B"""
+        import struct
+        t = len(indices)
+        assert len(points) == 32 * t
+        return self.call_host("b2k_ed25519_recover_commit", t, struct.pack("<%dI" % t, *indices), points, 32)
+
+    def ed25519_pubpoly_eval(self, commits: bytes, indices) -> bytes:
+        """PubPoly.Eval for every index: sum_j (I+1)^j C_j; commits [t][32] -> [n][32]"""
+        import struct
+        t, n = len(commits) // 32, len(indices)
+        out = bytearray(32 * n)
+        bufs = [_buf(x) for x in (commits, struct.pack("<%dI" % n, *indices), out)]
+        self._check(self.lib.b2k_ed25519_pubpoly_eval(self.h, t, bufs[0][0], n, bufs[1][0], bufs[2][0]))
+        return bytes(out)
+
+    def ed25519_pubpoly_check(self, commits: bytes, t: int, indices, shares_le: bytes) -> bytes:
+        """PubPoly.Check for m dealers x n shares: commits [m][t][32], indices m rows of n, shares [m][n][32] little-endian
+        -> m*n bytes (1 = the share matches the dealer's commitments)"""
+        import struct
+        m = len(commits) // (32 * t)
+        flat = [i for row in indices for i in row]
+        n = len(flat) // m
+        assert len(commits) == m * t * 32 and len(flat) == m * n and len(shares_le) == 32 * m * n
+        out = bytearray(m * n)
+        bufs = [_buf(x) for x in (commits, struct.pack("<%dI" % (m * n), *flat), shares_le, out)]
+        self._check(self.lib.b2k_ed25519_pubpoly_check(self.h, m, t, bufs[0][0], n, bufs[1][0], bufs[2][0], bufs[3][0]))
+        return bytes(out)
 
     def ed25519_verify(self, pks: bytes, msgs, sigs: bytes) -> bytes:
         """n x eddsa.VerifyWithChecks: pks [n][32], msgs list of bytes, sigs [n][64] R || s -> one status byte each

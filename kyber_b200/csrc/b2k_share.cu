@@ -9,45 +9,10 @@
 #define B2K_FP2_BYREF 1   // Fp2 products out of line BY REFERENCE (tower.cuh): instantiates the G2 MSM kernels (RecoverCommit on G2): same layout as b2k_g2.cu, or the weak host stubs of the two units would name different device code
 #include "msm_host.cuh"
 #include "codec.cuh"
+#include "lagrange.cuh"
 using namespace b2k_host;
 
 namespace b2k {
-
-// lambda_i = prod_{j != i} x_j / (x_j - x_i)  mod r, written as 32-byte big-endian scalars
-template <class FR>
-__global__ void __launch_bounds__(128) k_lagrange_at_zero(uint32_t t, const uint32_t* __restrict__ idx,
-                                                          uint8_t* __restrict__ scalars, uint32_t* flags) {
-  using S = Fp<FR>;
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= t) return;
-  S num, den, xi, xj, d;
-  fp_set_one(num);
-  fp_set_one(den);
-  fp_set_zero(xi);
-  const uint32_t ii = idx[i];
-  xi.v[0] = ii + 1u; xi.v[1] = (ii == 0xffffffffu) ? 1u : 0u;
-  fp_to_mont(xi, xi);
-  for (uint32_t j = 0; j < t; j++) {
-    if (j == i) continue;
-    const uint32_t jj = idx[j];
-    if (jj == ii) atomicOr(flags, 4u);          // duplicate index: denominator would be zero
-    fp_set_zero(xj);
-    xj.v[0] = jj + 1u; xj.v[1] = (jj == 0xffffffffu) ? 1u : 0u;
-    fp_to_mont(xj, xj);
-    fp_mul(num, num, xj);
-    fp_sub(d, xj, xi);
-    fp_mul(den, den, d);
-  }
-  fp_inv(den, den);
-  fp_mul(num, num, den);
-  fp_from_mont(num, num);
-  uint8_t* out = scalars + 32 * (size_t)i;
-#pragma unroll
-  for (int k = 0; k < 8; k++) {
-    uint8_t* q = out + 4 * (7 - k);
-    q[0] = (uint8_t)(num.v[k] >> 24); q[1] = (uint8_t)(num.v[k] >> 16); q[2] = (uint8_t)(num.v[k] >> 8); q[3] = (uint8_t)num.v[k];
-  }
-}
 
 // v = sum_j x^j C_j  (Horner: v = x v + C_j, poly.go:343-346), x * v by double-and-add over the bits of x (top bit consumed).
 // Out of line: inlined into k_pubpoly_check next to its scalar multiplication, sm_90a code gave wrong G2 points for t >= 2.
