@@ -480,6 +480,44 @@ int b2k_ed25519_pubpoly_eval(b2k_ctx* ctx, size_t t, const uint8_t* commits /*[t
 int b2k_ed25519_pubpoly_check(b2k_ctx* ctx, size_t m, size_t t, const uint8_t* commits /*[m][t][32]*/, size_t n,
                               const uint32_t* indices /*[m][n]*/, const uint8_t* shares /*[m][n][32] LE*/, uint8_t* ok /*[m][n]*/);
 
+/* ---- edwards25519 DLEQ proofs and PVSS ----------------------------------------------------------------------------------
+ * One status byte per proof, in the reference's order of failure:
+ *   B2K_DLEQ_POINT      an operand (point argument, VG or VH) does not decode like FromBytes: the reference could not have
+ *                       built this input
+ *   B2K_DLEQ_CHALLENGE  C differs from the expected challenge as raw bytes (Scalar.Equal, scalar.go:37-45): a C congruent to
+ *                       it but not canonical fails here
+ *   B2K_DLEQ_INVALID    VG != R G + C xG or VH != R H + C xH (dleq.Proof.Verify, proof/dleq/dleq.go:161-172)
+ * Proofs are 128 bytes C || R || VG || VH.  C and R are 32-byte little-endian, read raw as Point.Mul reads them (no reduction
+ * mod l; a top signed nibble above 8 selects nothing, as in b2k_ed25519_msm).  Points decode like FromBytes (non-canonical y
+ * accepted; all-zero bytes are the point of order 4).  Challenges hash MarshalTo of the DECODED points (their canonical
+ * encodings), SHA-256, then Scalar.Pick from blake2xb.New(digest) (the digest is the BLAKE2b key).
+ * Bad data is never a call error, only a status; B2K_ERR_ARG means a null pointer, a zero size, or m n or m t >= 2^31. */
+enum { B2K_DLEQ_OK = 0, B2K_DLEQ_CHALLENGE = 1, B2K_DLEQ_INVALID = 2, B2K_DLEQ_POINT = 3 };
+/* status[i] of dleq.Proof.Verify(g[i], h[i], xg[i], xh[i]) for n proofs (OK, INVALID or POINT).
+ * replaces: dleq.Proof.Verify called once per proof (dleq.go:161-172). */
+int b2k_ed25519_dleq_verify(b2k_ctx* ctx, size_t n, const uint8_t* g /*[n][32]*/, const uint8_t* h /*[n][32]*/,
+                            const uint8_t* xg /*[n][32]*/, const uint8_t* xh /*[n][32]*/, const uint8_t* proofs /*[n][128]*/,
+                            uint8_t* status /*[n]*/);
+/* device pointers; enqueue only */
+int b2k_ed25519_dleq_verify_dev(b2k_ctx* ctx, size_t n, const void* d_g, const void* d_h, const void* d_xg, const void* d_xh,
+                                const void* d_proofs, void* d_status);
+/* pvss.VerifyEncShareBatch (share/pvss/pvss.go:168-194) for m deals of n encrypted shares each, threshold t: deal d has the
+ * base h[d], the commitments commits[d][0..t), and per share i the key x[d][i], the caller's sH sh[d][i], the encrypted share
+ * v[d][i] and its proof.  The deal's challenge is Pick(XOF(SHA-256(coms[0..n) || V[0..n) || VG[0..n) || VH[0..n)))) with
+ * coms[i] = sum_j (i + 1)^j commits[d][j] at the POSITION i (pvss.go:94-149); each share then checks C against it and
+ * Verify(h, x, sh, v).  A deal whose h, a commitment, a V, VG or VH does not decode gives B2K_DLEQ_POINT for every share; an x or
+ * sh that does not decode only for its share.  K and E of the reference are the shares with status B2K_DLEQ_OK. */
+int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t n, const uint8_t* h /*[m][32]*/,
+                                       const uint8_t* commits /*[m][t][32]*/, const uint8_t* x /*[m][n][32]*/,
+                                       const uint8_t* sh /*[m][n][32]*/, const uint8_t* v /*[m][n][32]*/,
+                                       const uint8_t* proofs /*[m][n][128]*/, uint8_t* status /*[m][n]*/);
+/* pvss.VerifyDecShareBatch (pvss.go:281-299): per share, C against Pick(XOF(SHA-256(x || enc_v || VG || VH))), then
+ * Verify(g, dec_v, x, enc_v) (VerifyDecShare, pvss.go:248-277).  pvss.RecoverSecret is this call followed by
+ * b2k_ed25519_recover_commit on the shares with status B2K_DLEQ_OK (sorted by index, the first t). */
+int b2k_ed25519_pvss_verify_dec_shares(b2k_ctx* ctx, size_t n, const uint8_t* g /*[32]*/, const uint8_t* x /*[n][32]*/,
+                                       const uint8_t* enc_v /*[n][32]*/, const uint8_t* dec_v /*[n][32]*/,
+                                       const uint8_t* proofs /*[n][128]*/, uint8_t* status /*[n]*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

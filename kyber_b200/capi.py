@@ -70,6 +70,10 @@ def load_library() -> C.CDLL:
     sigs["b2k_ed25519_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
     sigs["b2k_ed25519_pubpoly_eval"] = (C.c_int, [vp, sz, vp, sz, vp, vp])
     sigs["b2k_ed25519_pubpoly_check"] = (C.c_int, [vp, sz, sz, vp, sz, vp, vp, vp])
+    sigs["b2k_ed25519_dleq_verify"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_dleq_verify_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_pvss_verify_enc_shares"] = (C.c_int, [vp, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_pvss_verify_dec_shares"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -563,6 +567,47 @@ class Engine:
         """the same on device pointers ([n][32], message bytes, [n+1] uint32 offsets, [n][64], [n] status); enqueue only"""
         self._check(self.lib.b2k_ed25519_verify_dev(self.h, n, C.c_void_p(d_pks), C.c_void_p(d_msgs), C.c_void_p(d_offsets),
                                                     C.c_void_p(d_sigs), C.c_void_p(d_status)))
+
+    def _status_call(self, name: str, n: int, sizes, ins, out_len: int) -> bytes:
+        status = bytearray(out_len)
+        bufs = [_buf(x) for x in (*ins, status)]
+        self._check(getattr(self.lib, name)(self.h, *sizes, *[b[0] for b in bufs]))
+        return bytes(status)
+
+    def ed25519_dleq_verify(self, g: bytes, h: bytes, xg: bytes, xh: bytes, proofs: bytes) -> bytes:
+        """n x dleq.Proof.Verify(G, H, xG, xH): points [n][32], proofs [n][128] C || R || VG || VH -> one status byte each
+        (B2K_DLEQ_*: 0 OK, 2 INVALID, 3 POINT)"""
+        n = len(g) // 32
+        assert len(g) == len(h) == len(xg) == len(xh) == 32 * n and len(proofs) == 128 * n
+        return self._status_call("b2k_ed25519_dleq_verify", n, (n,), (g, h, xg, xh, proofs), n)
+
+    def ed25519_dleq_verify_dev(self, n: int, d_g: int, d_h: int, d_xg: int, d_xh: int, d_proofs: int, d_status: int):
+        """the same on device pointers; enqueue only"""
+        self._check(self.lib.b2k_ed25519_dleq_verify_dev(self.h, n, *[C.c_void_p(p) for p in (d_g, d_h, d_xg, d_xh, d_proofs, d_status)]))
+
+    def ed25519_pvss_verify_enc_shares(self, h: bytes, commits: bytes, t: int, x: bytes, sh: bytes, v: bytes, proofs: bytes) -> bytes:
+        """pvss.VerifyEncShareBatch for m deals: h [m][32], commits [m][t][32], x, sh, v [m][n][32], proofs [m][n][128]
+        -> m*n status bytes (B2K_DLEQ_*)"""
+        m = len(h) // 32
+        n = len(x) // (32 * m)
+        assert len(h) == 32 * m and len(commits) == 32 * m * t
+        assert len(x) == len(sh) == len(v) == 32 * m * n and len(proofs) == 128 * m * n
+        return self._status_call("b2k_ed25519_pvss_verify_enc_shares", m * n, (m, t, n), (h, commits, x, sh, v, proofs), m * n)
+
+    def ed25519_pvss_verify_dec_shares(self, g: bytes, x: bytes, enc_v: bytes, dec_v: bytes, proofs: bytes) -> bytes:
+        """pvss.VerifyDecShareBatch: g [32], x, enc_v, dec_v [n][32], proofs [n][128] -> n status bytes (B2K_DLEQ_*)"""
+        n = len(x) // 32
+        assert len(g) == 32 and len(x) == len(enc_v) == len(dec_v) == 32 * n and len(proofs) == 128 * n
+        return self._status_call("b2k_ed25519_pvss_verify_dec_shares", n, (n,), (g, x, enc_v, dec_v, proofs), n)
+
+    def ed25519_pvss_recover_secret(self, g: bytes, indices, x: bytes, enc_v: bytes, dec_v: bytes, proofs: bytes, t: int):
+        """pvss.RecoverSecret (pvss.go:303-323): VerifyDecShareBatch, then RecoverCommit over the valid shares (sorted by index,
+        the first t, as xyCommit selects them) -> the 32-byte secret commitment, or None below t valid shares (ErrTooFewShares)"""
+        status = self.ed25519_pvss_verify_dec_shares(g, x, enc_v, dec_v, proofs)
+        good = sorted((indices[i], i) for i in range(len(status)) if status[i] == 0)[:t]
+        if len(good) < t or t == 0:
+            return None
+        return self.ed25519_recover_commit([idx for idx, _ in good], b"".join(dec_v[32 * i:32 * i + 32] for _, i in good))
 
     def bn254_pair(self, g1: bytes, g2: bytes) -> bytes:
         n = len(g1) // 64

@@ -79,18 +79,25 @@ B2K_D bool ed_decode(EdExt& r, const uint8_t* b) {
   return true;
 }
 
-// ToBytes (ge.go:99-107)
-B2K_D void ed_encode(uint8_t* out, const EdExt& p) {
-  EFp zi, x, y;
-  fp_inv(zi, p.Z);
-  fp_mul(x, p.X, zi); fp_mul(y, p.Y, zi);
-  fp_from_mont(x, x); fp_from_mont(y, y);
+// ToBytes of a point with Z = 1 (as ed_decode leaves it): the canonical encoding, no inversion
+B2K_D void ed_encode_z1(uint8_t* out, const EdExt& p) {
+  EFp x, y;
+  fp_from_mont(x, p.X); fp_from_mont(y, p.Y);
   y.v[7] |= (x.v[0] & 1u) << 31;
 #pragma unroll
   for (int j = 0; j < 8; j++) {
     out[4 * j] = (uint8_t)y.v[j]; out[4 * j + 1] = (uint8_t)(y.v[j] >> 8);
     out[4 * j + 2] = (uint8_t)(y.v[j] >> 16); out[4 * j + 3] = (uint8_t)(y.v[j] >> 24);
   }
+}
+
+// ToBytes (ge.go:99-107)
+B2K_D void ed_encode(uint8_t* out, const EdExt& p) {
+  EFp zi;
+  EdExt a;
+  fp_inv(zi, p.Z);
+  fp_mul(a.X, p.X, zi); fp_mul(a.Y, p.Y, zi);
+  ed_encode_z1(out, a);
 }
 
 // out = k * P, k the raw little-endian 256-bit integer
