@@ -518,6 +518,42 @@ int b2k_ed25519_pvss_verify_dec_shares(b2k_ctx* ctx, size_t n, const uint8_t* g 
                                        const uint8_t* enc_v /*[n][32]*/, const uint8_t* dec_v /*[n][32]*/,
                                        const uint8_t* proofs /*[n][128]*/, uint8_t* status /*[n]*/);
 
+/* ---- edwards25519 Neff shuffle verification (shuffle/) ------------------------------------------------------------------
+ * One status byte per shuffle, in the reference's order of failure:
+ *   B2K_SHUFFLE_POINT   an input point (g, h, x, y, xbar, ybar) or a proof point does not decode like FromBytes: the proof's Get
+ *                       fails (point.go:65) before any equation is checked
+ *   B2K_SHUFFLE_SIMPLE  a thver check of SimpleShuffle.Verify fails: "incorrect SimpleShuffleProof" (shuffle/simple.go:186-254)
+ *   B2K_SHUFFLE_PAIR    (33), (34) or (35) of PairShuffle.Verify fails: "invalid PairShuffleProof" (shuffle/pair.go:291-309)
+ * A proof is the fixbuf encoding of the prover's messages, fields in declaration order, no length prefixes, 32 bytes per item:
+ *   ega1 Gamma, A[k], C[k], U[k], W[k], Lambda1, Lambda2 | ega3 D[k] | ega5 Zsigma[k], Ztau | ssa0 X[k], Y[k] | ssa2 Theta[2k] |
+ *   ssa4 Zalpha[2k - 1]   = 32 (12k + 3) bytes.
+ * The transcript is proof.HashVerify's (proof/hash.go:92-142) with suite edwards25519.NewBlakeSHA256Ed25519: blake2xb.New(proto);
+ * each PubRand Reseeds (128 stream bytes -> New(them), xof/blake2xb/blake.go:55-75) and absorbs the RAW proof bytes read since the
+ * last one (ega1; ega3; ega5 || ssa0; ssa2 -- ssa4 and the inputs are not hashed); scalars are Scalar.Pick draws.  Proof
+ * scalars (Zsigma, Ztau, Zalpha) are read raw (no reduction mod l, scalar.go:226-232; a top signed nibble above 8 selects
+ * nothing, as in b2k_ed25519_msm).  Non-canonical point encodings are accepted; equality is exact point equality.
+ * The transcript runs on host threads inside the call (it needs the proof bytes on the host, so there is no _dev form).
+ * Bad data is never a call error, only a status.  B2K_ERR_ARG: a null pointer (proto may be null when proto_len = 0), k < 2,
+ * or m, k or m k above B2K_SHUFFLE_MAX_PAIRS. */
+#define B2K_SHUFFLE_MAX_PAIRS ((size_t)1 << 22)
+enum { B2K_SHUFFLE_OK = 0, B2K_SHUFFLE_SIMPLE = 1, B2K_SHUFFLE_PAIR = 2, B2K_SHUFFLE_POINT = 3 };
+/* status[s] of proof.HashVerify(suite, proto, shuffle.Verifier(suite, G, H, X[s], Y[s], Xbar[s], Ybar[s]), proofs[s]) for m
+ * shuffles of k >= 2 pairs (proof/hash.go:168-175, shuffle/pair.go:369-377); g, h: NULL = the base point, else [m][32].
+ * replaces: proof.HashVerify of one shuffle proof at a time (e.g. examples/neff_shuffle_test.go). */
+int b2k_ed25519_shuffle_verify(b2k_ctx* ctx, size_t m, size_t k, const uint8_t* g /*[m][32] or NULL*/,
+                               const uint8_t* h /*[m][32] or NULL*/, const uint8_t* x /*[m][k][32]*/, const uint8_t* y /*[m][k][32]*/,
+                               const uint8_t* xbar /*[m][k][32]*/, const uint8_t* ybar /*[m][k][32]*/,
+                               const uint8_t* proofs /*[m][32 (12k + 3)]*/, const uint8_t* proto, uint32_t proto_len,
+                               uint8_t* status /*[m]*/);
+/* shuffle.GetSequenceVerifiable (shuffle/sequences.go:155-190): x_up[i] = sum_j e[j] x[j][i], and y_up, x_down (xbar), y_down
+ * (ybar) likewise, as canonical encodings.  e [nq][32] little-endian, read raw like any Point.Mul scalar.  A point that does not
+ * decode -> B2K_ERR_POINT.  B2K_ERR_ARG: a null pointer, nq or k zero, or nq, k or nq k above B2K_SHUFFLE_MAX_PAIRS. */
+int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, const uint8_t* x /*[nq][k][32]*/,
+                                            const uint8_t* y /*[nq][k][32]*/, const uint8_t* xbar /*[nq][k][32]*/,
+                                            const uint8_t* ybar /*[nq][k][32]*/, const uint8_t* e /*[nq][32]*/,
+                                            uint8_t* x_up /*[k][32]*/, uint8_t* y_up /*[k][32]*/, uint8_t* x_down /*[k][32]*/,
+                                            uint8_t* y_down /*[k][32]*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

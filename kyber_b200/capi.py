@@ -74,6 +74,8 @@ def load_library() -> C.CDLL:
     sigs["b2k_ed25519_dleq_verify_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
     sigs["b2k_ed25519_pvss_verify_enc_shares"] = (C.c_int, [vp, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp])
     sigs["b2k_ed25519_pvss_verify_dec_shares"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_shuffle_verify"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp])
+    sigs["b2k_ed25519_shuffle_sequence_verifiable"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -608,6 +610,29 @@ class Engine:
         if len(good) < t or t == 0:
             return None
         return self.ed25519_recover_commit([idx for idx, _ in good], b"".join(dec_v[32 * i:32 * i + 32] for _, i in good))
+
+    def ed25519_shuffle_verify(self, k: int, x: bytes, y: bytes, xbar: bytes, ybar: bytes, proofs: bytes,
+                               proto: bytes = b"", g: bytes = None, h: bytes = None) -> bytes:
+        """m x proof.HashVerify(suite, proto, shuffle.Verifier(suite, G, H, X, Y, Xbar, Ybar), proof): x, y, xbar, ybar
+        [m][k][32], proofs [m][32 (12k + 3)], g / h None (the base point) or [m][32] -> m status bytes (B2K_SHUFFLE_*: 0 OK,
+        1 SIMPLE, 2 PAIR, 3 POINT)"""
+        m = len(x) // (32 * k)
+        assert m > 0 and len(x) == len(y) == len(xbar) == len(ybar) == 32 * m * k and len(proofs) == 32 * (12 * k + 3) * m
+        assert (g is None or len(g) == 32 * m) and (h is None or len(h) == 32 * m)
+        status = bytearray(m)
+        bufs = [_buf(b) if b is not None else (None, None) for b in (g, h, x, y, xbar, ybar, proofs, bytes(proto), status)]
+        self._check(self.lib.b2k_ed25519_shuffle_verify(self.h, m, k, *[b[0] for b in bufs[:8]], len(proto), bufs[8][0]))
+        return bytes(status)
+
+    def ed25519_shuffle_sequence_verifiable(self, nq: int, x: bytes, y: bytes, xbar: bytes, ybar: bytes, e: bytes):
+        """shuffle.GetSequenceVerifiable: x, y, xbar, ybar [nq][k][32], e [nq][32] little-endian (raw) -> (xUp, yUp, xDown,
+        yDown), each [k][32] canonical encodings"""
+        k = len(x) // (32 * nq)
+        assert k > 0 and len(x) == len(y) == len(xbar) == len(ybar) == 32 * nq * k and len(e) == 32 * nq
+        outs = [bytearray(32 * k) for _ in range(4)]
+        bufs = [_buf(b) for b in (x, y, xbar, ybar, e, *outs)]
+        self._check(self.lib.b2k_ed25519_shuffle_sequence_verifiable(self.h, nq, k, *[b[0] for b in bufs]))
+        return tuple(bytes(o) for o in outs)
 
     def bn254_pair(self, g1: bytes, g2: bytes) -> bytes:
         n = len(g1) // 64

@@ -12,9 +12,13 @@
 #if defined(__CUDACC__)
 #define B2K_D __device__ __forceinline__
 #define B2K_NI static __device__ __noinline__
+#define B2K_HD __host__ __device__ __forceinline__        // also called by host code of a .cu unit (the shuffle transcript)
+#define B2K_HNI static __host__ __device__ __noinline__
 #else
 #define B2K_D inline
 #define B2K_NI inline
+#define B2K_HD inline
+#define B2K_HNI inline
 #ifndef B2K_HOST_EMUL
 #define B2K_HOST_EMUL 1
 #endif

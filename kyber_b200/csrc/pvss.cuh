@@ -24,8 +24,9 @@ namespace b2k {
 enum { DLEQ_OK = 0, DLEQ_CHALLENGE = 1, DLEQ_INVALID = 2, DLEQ_POINT = 3 };
 
 // ---- BLAKE2b (RFC 7693) and BLAKE2Xb ------------------------------------------------------------------------------------
+// host-callable too (B2K_HD): the shuffle verifier runs its Fiat-Shamir transcript on host threads with this same code
 struct Blake2bSigma {
-  B2K_D static int s(int r, int i) {
+  B2K_HD static int s(int r, int i) {
     constexpr uint8_t t[10][16] = {{0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15}, {14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3},
                                    {11, 8, 12, 0, 5, 2, 15, 13, 10, 14, 3, 6, 7, 1, 9, 4}, {7, 9, 3, 1, 13, 12, 11, 14, 2, 6, 5, 10, 4, 0, 15, 8},
                                    {9, 0, 5, 7, 2, 4, 10, 15, 14, 1, 11, 12, 6, 8, 3, 13}, {2, 12, 6, 10, 0, 11, 8, 3, 4, 13, 7, 5, 15, 14, 1, 9},
@@ -33,9 +34,14 @@ struct Blake2bSigma {
                                    {6, 15, 14, 9, 11, 3, 0, 8, 12, 2, 13, 7, 1, 4, 10, 5}, {10, 2, 8, 4, 7, 6, 1, 5, 15, 11, 9, 14, 3, 12, 13, 0}};
     return t[r % 10][i];
   }
+  B2K_HD static uint64_t iv(int j) {                    // BLAKE2b's IV is SHA-512's
+    constexpr uint64_t t[8] = {0x6a09e667f3bcc908ull, 0xbb67ae8584caa73bull, 0x3c6ef372fe94f82bull, 0xa54ff53a5f1d36f1ull,
+                               0x510e527fade682d1ull, 0x9b05688c2b3e6c1full, 0x1f83d9abfb41bd6bull, 0x5be0cd19137e2179ull};
+    return t[j];
+  }
 };
 
-B2K_D void blake2b_g(uint64_t* v, int a, int b, int c, int d, uint64_t x, uint64_t y) {
+B2K_HD void blake2b_g(uint64_t* v, int a, int b, int c, int d, uint64_t x, uint64_t y) {
   v[a] = v[a] + v[b] + x; v[d] = sha_rotr(v[d] ^ v[a], 32);
   v[c] = v[c] + v[d]; v[b] = sha_rotr(v[b] ^ v[c], 24);
   v[a] = v[a] + v[b] + y; v[d] = sha_rotr(v[d] ^ v[a], 16);
@@ -43,10 +49,10 @@ B2K_D void blake2b_g(uint64_t* v, int a, int b, int c, int d, uint64_t x, uint64
 }
 
 // one compression of the 16 little-endian message words m; t = bytes hashed so far including this block (< 2^64 here)
-B2K_NI void blake2b_compress(uint64_t* h, const uint64_t* m, uint64_t t, bool last) {
+B2K_HNI void blake2b_compress(uint64_t* h, const uint64_t* m, uint64_t t, bool last) {
   uint64_t v[16];
 #pragma unroll
-  for (int i = 0; i < 8; i++) { v[i] = h[i]; v[i + 8] = Sha512K::iv(i); }   // BLAKE2b's IV is SHA-512's
+  for (int i = 0; i < 8; i++) { v[i] = h[i]; v[i + 8] = Blake2bSigma::iv(i); }
   v[12] ^= t;
   if (last) v[14] = ~v[14];
 #pragma unroll
@@ -65,9 +71,9 @@ B2K_NI void blake2b_compress(uint64_t* h, const uint64_t* m, uint64_t t, bool la
 }
 
 // h = IV xor the parameter block, whose words 0..2 are given (the rest is zero in every use here)
-B2K_D void blake2b_init(uint64_t* h, uint64_t p0, uint64_t p1, uint64_t p2) {
+B2K_HD void blake2b_init(uint64_t* h, uint64_t p0, uint64_t p1, uint64_t p2) {
 #pragma unroll
-  for (int i = 0; i < 8; i++) h[i] = Sha512K::iv(i);
+  for (int i = 0; i < 8; i++) h[i] = Blake2bSigma::iv(i);
   h[0] ^= p0; h[1] ^= p1; h[2] ^= p2;
 }
 
@@ -97,7 +103,7 @@ B2K_D void blake2xb_root(uint64_t* h0, const uint8_t* seed, uint32_t len) {
 
 // output block i of the XOF (64 bytes as 8 little-endian words): unkeyed BLAKE2b-512 of the 64-byte root hash with the BLAKE2X
 // node parameters: leaf length 64, node offset i, XOF length 2^32 - 1, inner length 64
-B2K_D void blake2xb_block(uint64_t* out, const uint64_t* h0, uint32_t i) {
+B2K_HD void blake2xb_block(uint64_t* out, const uint64_t* h0, uint32_t i) {
   blake2b_init(out, 64ull | (64ull << 32), (uint64_t)i | (0xffffffffull << 32), 64ull << 8);
   uint64_t m[16];
 #pragma unroll
