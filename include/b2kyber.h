@@ -299,7 +299,8 @@ int b2k_bls12381_pairing_check_dev(b2k_ctx* ctx, size_t n, const void* d_a1, con
  * (pairing/bls12381/kilic/gt.go:33-83; pairing/bn254/point.go:560-623).  Elements travel as their MarshalBinary bytes
  * (BLS12-381: 576 B, kilic/gt.go:115-117; bn254/bn256: 384 B, pairing/bn254/point.go:625-656); a coefficient >= p raises
  * B2K_ERR_POINT where the reference's Unmarshal range-checks (BLS12-381, bn254).  gt_exp takes 32-byte big-endian scalars
- * below the group order and is valid for any Fp12 element (plain square-and-multiply).
+ * below the group order and is valid for any Fp12 element (plain square-and-multiply).  gt_inv maps the zero element (all
+ * coefficients 0, not a member of GT) to zero, as the field inversion underneath maps 0 to 0.
  * miller / final_exp (finalize): pointGT.Miller and pointGT.Finalize (pairing/bn254/point.go:768-786) -- exported by the
  * reference so that a caller can multiply several Miller values and pay ONE final exponentiation; miller(...) output fed to
  * final_exp(...) equals pair(...).  An operand at infinity gives 1 (pairing/bn254/optate.go:267-269).

@@ -337,6 +337,7 @@ template <class C>
 B2K_D void fp_mul_inl(Fp<C>& r, const Fp<C>& a, const Fp<C>& b) {
   constexpr int N = C::N;
   static_assert(N % 2 == 0, "even limb count");
+  static_assert(C::BITS <= 32 * C::N - 1, "p < 2^(32N-1): the merged rows and fp_reduce_once carry nothing out of the top limb");
   uint32_t ev[N], od[N];
 #pragma unroll
   for (int i = 0; i < N; i += 2) {
@@ -435,6 +436,7 @@ B2K_NI void fp_sqr_c(Fp<C>& r, const Fp<C>& a) { fp_sqr(r, a); }
 template <class C>
 B2K_D void fp_add(Fp<C>& r, const Fp<C>& a, const Fp<C>& b) {
   constexpr int N = C::N;
+  static_assert(C::BITS <= 32 * C::N - 1, "p < 2^(32N-1): the sum of two operands below p has no carry out of the top limb");
   uint32_t t[N];
   t[0] = ptx::add_cc(a.v[0], b.v[0]);
 #pragma unroll
