@@ -293,6 +293,40 @@ int b2k_bls12381_pairing_check(b2k_ctx* ctx, size_t n, const uint8_t* a1 /*[n][9
                                const uint8_t* b1 /*[n][96]*/, const uint8_t* b2 /*[n][192]*/, uint8_t* ok /*[n]*/);
 int b2k_bls12381_pairing_check_dev(b2k_ctx* ctx, size_t n, const void* d_a1, const void* d_a2, const void* d_b1,
                                    const void* d_b2, void* d_ok);
+/* gt[i] = e(g1[i], g2) for ONE g2 operand: its Miller-loop lines are computed once and shared by every element (the kernel
+ * b2k_bls12381_ibe_decrypt_cca_g1 runs above the cooperative size).  Same bytes as b2k_bls12381_pair with g2 repeated n times. */
+int b2k_bls12381_pair_fixed_g2(b2k_ctx* ctx, size_t n, const uint8_t* g1 /*[n][96]*/, const uint8_t* g2 /*[192]*/,
+                               uint8_t* gt /*[n][576]*/);
+
+/* ---- encrypt/ibe: Boneh-Franklin CCA encryption on BLS12-381 ---------------------------------------------------------------
+ * One key (or master key and identity) and n messages of one length len, 0 <= len <= 32 (s.Hash().Size(), SHA-256); points are
+ * compressed kyber wire bytes.  With len bytes of each hash:
+ *   H2(g) = SHA256("IBE-H2" || GT.MarshalBinary(g)),  H4(sigma) = SHA256("IBE-H4" || sigma),
+ *   H3(sigma, msg): buf = SHA256("IBE-H3" || sigma || msg); for i = 1 .. 65534: h = SHA256(LE16(i) || buf), h[0] >>= 1, the
+ *   first h < r read big-endian.
+ * Decrypt: sigma = V xor H2(e(U, priv)) (OnG2: e(priv, U)), msg = W xor H4(sigma), accepted when H3(sigma, msg) Base == U.
+ * status[i]: B2K_IBE_OK, B2K_IBE_PROOF (the reference's "invalid proof: rP check failed"; U at infinity gives this), or
+ * B2K_IBE_POINT (U does not decode with the checks of b2k_bls12381_g1/g2_decompress); msg[i] is zeroed unless OK.
+ * Encrypt: Gid = e(master, Q_id) (OnG2: e(Q_id, master)) with Q_id = hash_to_g2(id) (OnG2: hash_to_g1), dst NULL = the default
+ * DST of that hash; for each message r = H3(sigma, msg), U = r Base, V = sigma xor H2(Gid^r), W = msg xor H4(sigma).  sigma is
+ * the caller's randomness (crypto/rand in the reference).
+ * A key that does not decode -> B2K_ERR_POINT; len > 32, n = 0 or a null pointer -> B2K_ERR_ARG.  Blocking, host buffers.
+ *   replaces: DecryptCCAonG1 ibe.go:99-134, DecryptCCAonG2 ibe.go:196-231, EncryptCCAonG1 ibe.go:51-97, EncryptCCAonG2 ibe.go:148-194 */
+enum { B2K_IBE_OK = 0, B2K_IBE_PROOF = 1, B2K_IBE_POINT = 2 };
+int b2k_bls12381_ibe_decrypt_cca_g1(b2k_ctx* ctx, const uint8_t* priv /*[96]*/, size_t n, const uint8_t* u /*[n][48]*/, size_t len,
+                                    const uint8_t* v /*[n][len]*/, const uint8_t* w /*[n][len]*/, uint8_t* msg /*[n][len]*/,
+                                    uint8_t* status /*[n]*/);
+int b2k_bls12381_ibe_decrypt_cca_g2(b2k_ctx* ctx, const uint8_t* priv /*[48]*/, size_t n, const uint8_t* u /*[n][96]*/, size_t len,
+                                    const uint8_t* v /*[n][len]*/, const uint8_t* w /*[n][len]*/, uint8_t* msg /*[n][len]*/,
+                                    uint8_t* status /*[n]*/);
+int b2k_bls12381_ibe_encrypt_cca_g1(b2k_ctx* ctx, const uint8_t* master /*[48]*/, const uint8_t* id, size_t id_len, const uint8_t* dst,
+                                    size_t dst_len, size_t n, size_t len, const uint8_t* msgs /*[n][len]*/,
+                                    const uint8_t* sigmas /*[n][len]*/, uint8_t* u /*[n][48]*/, uint8_t* v /*[n][len]*/,
+                                    uint8_t* w /*[n][len]*/);
+int b2k_bls12381_ibe_encrypt_cca_g2(b2k_ctx* ctx, const uint8_t* master /*[96]*/, const uint8_t* id, size_t id_len, const uint8_t* dst,
+                                    size_t dst_len, size_t n, size_t len, const uint8_t* msgs /*[n][len]*/,
+                                    const uint8_t* sigmas /*[n][len]*/, uint8_t* u /*[n][96]*/, uint8_t* v /*[n][len]*/,
+                                    uint8_t* w /*[n][len]*/);
 
 /* ---- the target group as a kyber.Group, Miller / Finalize, products of pairings, G1 / G2 Add ------------------------------
  * GT is written additively in kyber: Add = Fp12 product, Neg = inverse, Mul = exponentiation, Null = 1

@@ -57,6 +57,10 @@ def load_library() -> C.CDLL:
     sigs["b2k_bls12381_pair_dev"] = (C.c_int, [vp, sz, vp, vp, vp])
     sigs["b2k_bls12381_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bls12381_pairing_check_dev"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
+    sigs["b2k_bls12381_pair_fixed_g2"] = (C.c_int, [vp, sz, vp, vp, vp])
+    for g in ("g1", "g2"):
+        sigs[f"b2k_bls12381_ibe_decrypt_cca_{g}"] = (C.c_int, [vp, vp, sz, vp, sz, vp, vp, vp, vp])
+        sigs[f"b2k_bls12381_ibe_encrypt_cca_{g}"] = (C.c_int, [vp, vp, vp, sz, vp, sz, sz, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bls12381_hash_to_g1"] = (C.c_int, [vp, sz, vp, vp, vp, C.c_uint32, vp])
     sigs["b2k_bls12381_hash_to_g1_dev"] = (C.c_int, [vp, sz, vp, vp, vp, C.c_uint32, vp])
     sigs["b2k_bls12381_hash_to_g2"] = (C.c_int, [vp, sz, vp, vp, vp, C.c_uint32, vp])
@@ -410,6 +414,42 @@ class Engine:
         n = len(g1) // 96
         assert len(g1) == 96 * n and len(g2) == 192 * n
         return self.call_host("b2k_bls12381_pair", n, g1, g2, 576 * n)
+
+    def bls12381_pair_fixed_g2(self, g1: bytes, g2: bytes) -> bytes:
+        """gt[i] = e(g1[i], g2) for one g2 operand [192] (its Miller-loop lines shared by every element)"""
+        n = len(g1) // 96
+        assert len(g1) == 96 * n and len(g2) == 192
+        return self.call_host("b2k_bls12381_pair_fixed_g2", n, g1, g2, 576 * n)
+
+    # -- encrypt/ibe: Boneh-Franklin CCA ---------------------------------------------------------------
+    def bls12381_ibe_decrypt(self, on: int, priv: bytes, u: bytes, v, w):
+        """n x DecryptCCAonG1 (on = 1: priv [96] on G2, u [n][48]) / DecryptCCAonG2 (on = 2: priv [48] on G1, u [n][96]); v, w lists
+        of n byte strings of one length <= 32 -> (list of n messages, status bytes [n] B2K_IBE_*: 0 OK, 1 PROOF, 2 POINT)"""
+        assert on in (1, 2) and len(priv) == 144 - 48 * on
+        n = len(v)
+        ln = len(v[0]) if n else 0
+        assert len(u) == 48 * on * n and len(w) == n and all(len(x) == ln for x in list(v) + list(w))
+        msg, status = bytearray(max(n * ln, 1)), bytearray(max(n, 1))
+        bufs = [_buf(x) for x in (priv, u or b"\x00", b"".join(v) or b"\x00", b"".join(w) or b"\x00", msg, status)]
+        self._check(getattr(self.lib, f"b2k_bls12381_ibe_decrypt_cca_g{on}")(self.h, bufs[0][0], n, bufs[1][0], ln, bufs[2][0], bufs[3][0],
+                                                                            bufs[4][0], bufs[5][0]))
+        return [bytes(msg[ln * i:ln * (i + 1)]) for i in range(n)], bytes(status[:n])
+
+    def bls12381_ibe_encrypt(self, on: int, master: bytes, ident: bytes, msgs, sigmas, dst: bytes = None):
+        """n x EncryptCCAonG1 (on = 1: master [48] on G1, U [n][48]) / EncryptCCAonG2 (on = 2: master [96] on G2, U [n][96]) towards
+        one identity; msgs, sigmas lists of n byte strings of one length <= 32; dst None = the default DST of the identity's hash
+        -> (u bytes [n][48 on], list of n V, list of n W)"""
+        assert on in (1, 2) and len(master) == 48 * on
+        n = len(msgs)
+        ln = len(msgs[0]) if n else 0
+        assert len(sigmas) == n and all(len(x) == ln for x in list(msgs) + list(sigmas))
+        u, v, w = bytearray(max(48 * on * n, 1)), bytearray(max(n * ln, 1)), bytearray(max(n * ln, 1))
+        bufs = [_buf(x) for x in (master, ident or b"\x00", dst or b"\x00", b"".join(msgs) or b"\x00", b"".join(sigmas) or b"\x00",
+                                  u, v, w)]
+        self._check(getattr(self.lib, f"b2k_bls12381_ibe_encrypt_cca_g{on}")(
+            self.h, bufs[0][0], bufs[1][0], len(ident), bufs[2][0] if dst is not None else None, len(dst) if dst is not None else 0,
+            n, ln, bufs[3][0], bufs[4][0], bufs[5][0], bufs[6][0], bufs[7][0]))
+        return bytes(u[:48 * on * n]), [bytes(v[ln * i:ln * (i + 1)]) for i in range(n)], [bytes(w[ln * i:ln * (i + 1)]) for i in range(n)]
 
     def bls12381_pairing_check(self, a1: bytes, a2: bytes, b1: bytes, b2: bytes) -> bytes:
         n = len(a1) // 96

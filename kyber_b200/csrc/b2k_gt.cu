@@ -303,6 +303,19 @@ __global__ void __launch_bounds__(128) k_add_batch(size_t n, const uint8_t* __re
 // ================================================================================================
 namespace {
 
+// out[i] = a[i]^scalars[i] on device buffers: one warp per element for small batches, one thread per element above
+template <class P>
+void launch_gt_exp(const b2k_ctx* ctx, size_t n, const uint8_t* ds, const uint8_t* da, uint8_t* dout) {
+  if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 4096 ? ctx->coop_max_n : 4096)) {
+    using SQR = typename P::CoopSqr;
+    using MUL = typename P::CoopMul;
+    using C = typename P::FC;
+    constexpr int NS = (SQR::SLOTS > MUL::SLOTS ? SQR::SLOTS : MUL::SLOTS) | 1;
+    k_coop_gt_exp<P, C, SQR, MUL><<<(unsigned)n, 32, (size_t)C::N * (NS + 12) * 4, ctx->stream>>>(n, ds, da, dout, ctx->d_flags);
+  } else
+    k_gt_exp<P><<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(n, ds, da, dout, ctx->d_flags);
+}
+
 template <class P>
 int gt_binary(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* a, const uint8_t* b, uint8_t* out, int op) {
   if (!ctx || !a || !out || n == 0 || (op == 0 && !b) || (op == 2 && !scalars)) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
@@ -326,14 +339,7 @@ int gt_binary(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* a, 
     k_gt_inv<P><<<grid, 64, 0, st>>>(n, da, dout, ctx->d_flags);
   } else {
     CK(cudaMemcpyAsync(ds, scalars, n * 32, cudaMemcpyHostToDevice, st));
-    if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 4096 ? ctx->coop_max_n : 4096)) {
-      using SQR = typename P::CoopSqr;
-      using MUL = typename P::CoopMul;
-      using C = typename P::FC;
-      constexpr int NS = (SQR::SLOTS > MUL::SLOTS ? SQR::SLOTS : MUL::SLOTS) | 1;
-      k_coop_gt_exp<P, C, SQR, MUL><<<(unsigned)n, 32, (size_t)C::N * (NS + 12) * 4, st>>>(n, ds, da, dout, ctx->d_flags);
-    } else
-      k_gt_exp<P><<<grid, 64, 0, st>>>(n, ds, da, dout, ctx->d_flags);
+    launch_gt_exp<P>(ctx, n, ds, da, dout);
   }
   CK(cudaGetLastError());
   ctx->launches += 1;
@@ -472,5 +478,10 @@ int b2k_bn256_pairing_product_check(b2k_ctx* c, size_t n, const uint8_t* g1, con
 
 int b2k_bls12381_g1_add_batch(b2k_ctx* c, size_t n, const uint8_t* a, const uint8_t* b, int neg, uint8_t* o) { return add_batch_host<Bls381G1>(c, n, a, b, neg, o); }
 int b2k_bls12381_g2_add_batch(b2k_ctx* c, size_t n, const uint8_t* a, const uint8_t* b, int neg, uint8_t* o) { return add_batch_host<Bls381G2>(c, n, a, b, neg, o); }
+
+// the exponentiation dispatch of b2k_bls12381_gt_exp on device buffers (the IBE encryption's Gid^r, b2k_ibe.cu); enqueue only
+void b2k_internal_launch_bls12381_gt_exp(const b2k_ctx* c, size_t n, const uint8_t* ds, const uint8_t* da, uint8_t* dout) {
+  launch_gt_exp<BlsPairing>(c, n, ds, da, dout);
+}
 
 }  // extern "C"
