@@ -589,6 +589,27 @@ int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, c
                                             uint8_t* x_up /*[k][32]*/, uint8_t* y_up /*[k][32]*/, uint8_t* x_down /*[k][32]*/,
                                             uint8_t* y_down /*[k][32]*/);
 
+/* ---- edwards25519 ring signatures (sign/anon) --------------------------------------------------------------------------
+ * status[j] of anon.Verify(suite, msg_j, ring, linkable ? scope : nil, sigs[j]) for m signatures over ONE ring and ONE
+ * scope; suite = edwards25519.NewBlakeSHA256Ed25519 (XOF = blake2xb).  sig_j = C0 || S_0..S_{n-1} [|| Tag] (32 (n + 1 +
+ * linkable) bytes; the caller cuts longer buffers and answers shorter ones itself, as fixbuf would).  tags (may be NULL):
+ * the canonical Tag of every OK linkable signature, zero otherwise.  A ring key that does not decode -> B2K_ERR_POINT;
+ * m == 0 or a null pointer -> B2K_ERR_ARG; n == 0 is legal (the reference's loop does not run).  Blocking, host buffers.
+ *   B2K_ANON_INVALID  the final challenge differs from C0: "invalid signature" (sig.go:242-244)
+ *   B2K_ANON_POINT    the Tag does not decode: "invalid Ed25519 curve point" (fixbuf's read of the Tag)
+ * Scalars are read raw (no reduction mod l; a top signed nibble above 8 selects nothing, as geScalarMult and
+ * geScalarMultBase do); C0 is compared as raw bytes (Scalar.Equal), so a C0 >= l never verifies when n >= 1.  A non-canonical
+ * Tag encoding that decodes is accepted; H1 hashes, and tags returns, its canonical encoding.  One signature is one thread's
+ * n-step chain: the batch is the use.  msgs/offsets as in b2k_ed25519_verify; ring may be NULL when n = 0, scope when
+ * scope_len = 0 or unlinkable.  B2K_ERR_ARG also for m, n, m (n + 2) or scope_len above B2K_ANON_MAX.
+ *   replaces: anon.Verify (sign/anon/sig.go:192-248) called once per signature */
+#define B2K_ANON_MAX ((size_t)1 << 30)
+enum { B2K_ANON_OK = 0, B2K_ANON_INVALID = 1, B2K_ANON_POINT = 2 };
+int b2k_ed25519_anon_verify(b2k_ctx* ctx, size_t n, const uint8_t* ring /*[n][32]*/, int linkable,
+                            const uint8_t* scope, size_t scope_len, size_t m, const uint8_t* msgs,
+                            const uint32_t* offsets /*[m+1]*/, const uint8_t* sigs, uint8_t* status /*[m]*/,
+                            uint8_t* tags /*[m][32] or NULL*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

@@ -80,6 +80,7 @@ def load_library() -> C.CDLL:
     sigs["b2k_ed25519_pvss_verify_dec_shares"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp, vp])
     sigs["b2k_ed25519_shuffle_verify"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp])
     sigs["b2k_ed25519_shuffle_sequence_verifiable"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_anon_verify"] = (C.c_int, [vp, sz, vp, C.c_int, vp, sz, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -673,6 +674,21 @@ class Engine:
         bufs = [_buf(b) for b in (x, y, xbar, ybar, e, *outs)]
         self._check(self.lib.b2k_ed25519_shuffle_sequence_verifiable(self.h, nq, k, *[b[0] for b in bufs]))
         return tuple(bytes(o) for o in outs)
+
+    def ed25519_anon_verify(self, ring: bytes, msgs, sigs, scope: bytes = None):
+        """m x anon.Verify(suite, msgs[j], ring, scope, sigs[j]) over one ring [n][32]: scope None = unlinkable, b"" = linkable
+        with an empty scope; sigs: list of m signatures of exactly 32 (n + 1 + linkable) bytes -> (m status bytes (B2K_ANON_*:
+        0 OK, 1 INVALID, 2 POINT), [m][32] tags: the canonical Tag of every OK linkable signature, zero otherwise)"""
+        n, m, linkable = len(ring) // 32, len(msgs), scope is not None
+        siglen = 32 * (n + 1 + linkable)
+        assert len(ring) == 32 * n and len(sigs) == m and all(len(s) == siglen for s in sigs)
+        blob, offs = self._pack_msgs(msgs)
+        status, tags = bytearray(m), bytearray(32 * m)
+        sc = bytes(scope or b"")
+        bufs = [_buf(x) if len(x) else (None, None) for x in (bytes(ring), sc, blob, offs, b"".join(sigs) or b"\x00", status, tags)]
+        self._check(self.lib.b2k_ed25519_anon_verify(self.h, n, bufs[0][0], int(linkable), bufs[1][0], len(sc), m,
+                                                     *[b[0] for b in bufs[2:]]))
+        return bytes(status), bytes(tags)
 
     def bn254_pair(self, g1: bytes, g2: bytes) -> bytes:
         n = len(g1) // 64

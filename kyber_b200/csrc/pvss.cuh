@@ -77,6 +77,43 @@ B2K_HD void blake2b_init(uint64_t* h, uint64_t p0, uint64_t p1, uint64_t p2) {
   h[0] ^= p0; h[1] ^= p1; h[2] ^= p2;
 }
 
+// A BLAKE2b midstate: the chaining value h, the bytes compressed so far t, and the pending block m of n <= 128 bytes (little-
+// endian words).  A full block is compressed only when more input arrives, so the last block can still take the final flag.
+struct Blake2bMid { uint64_t h[8]; uint64_t t; uint64_t m[16]; uint32_t n; };
+
+B2K_HD void blake2b_absorb(Blake2bMid& s, const uint8_t* p, uint32_t len) {
+  for (uint32_t k = 0; k < len; k++) {
+    if (s.n == 128) {
+      s.t += 128;
+      blake2b_compress(s.h, s.m, s.t, false);
+      for (int i = 0; i < 16; i++) s.m[i] = 0;
+      s.n = 0;
+    }
+    s.m[s.n >> 3] |= (uint64_t)p[k] << (8 * (s.n & 7));
+    s.n++;
+  }
+}
+
+// the 64-byte digest (8 little-endian words) of everything absorbed: the pending block compressed as the last one
+B2K_HD void blake2b_finish(uint64_t* out, const Blake2bMid& s) {
+  uint64_t m[16];
+  for (int i = 0; i < 16; i++) m[i] = s.m[i];
+  for (int i = 0; i < 8; i++) out[i] = s.h[i];
+  blake2b_compress(out, m, s.t + s.n, true);
+}
+
+// blake2xb.New(seed) as a midstate, to which XOF.Write appends (the same stream blake2xb_root hashes in one go)
+B2K_HD void blake2xb_begin(Blake2bMid& s, const uint8_t* seed, uint32_t len) {
+  const uint32_t klen = len < 64 ? len : 64;
+  blake2b_init(s.h, 64u | (klen << 8) | (1u << 16) | (1u << 24), 0xffffffffull << 32, 0);
+  s.t = 0;
+  s.n = 0;
+  for (int i = 0; i < 16; i++) s.m[i] = 0;
+  blake2b_absorb(s, seed, klen);
+  if (klen) s.n = 128;
+  blake2b_absorb(s, seed + klen, len - klen);
+}
+
 // The root hash of blake2xb.New(seed): BLAKE2b-512 KEYED with seed[0, min(len, 64)) over the message seed[64, len), with
 // fanout 1, depth 1 and the XOF length 2^32 - 1 (unknown) in the parameter block.  A key is hashed as a zero-padded first block.
 B2K_D void blake2xb_root(uint64_t* h0, const uint8_t* seed, uint32_t len) {
@@ -111,8 +148,33 @@ B2K_HD void blake2xb_block(uint64_t* out, const uint64_t* h0, uint32_t i) {
   blake2b_compress(out, m, 64, true);
 }
 
-// Scalar.Pick(blake2xb.New(seed)) as 8 little-endian limbs: random.Int(l) draws 32 stream bytes, clears the top 3 bits of the
-// first (l has 253 bits), reads them big-endian and draws again while the value is >= l.  An output block holds two draws.
+// Scalar.Pick of the XOF whose root hash is h0, as 8 little-endian limbs: random.Int(l) draws 32 stream bytes, clears the top 3
+// bits of the first (l has 253 bits), reads them big-endian and draws again while the value is >= l.  An output block holds two
+// draws.
+B2K_D void sc_pick_root(uint32_t* s, const uint64_t* h0) {
+  uint64_t blk[8];
+  for (uint32_t i = 0;; i++) {
+    blake2xb_block(blk, h0, i);
+    for (int half = 0; half < 2; half++) {
+#pragma unroll
+      for (int j = 0; j < 8; j++) {                     // limb j holds draw bytes 31 - 4 j - q (q = 0..3) at bits 8 q
+        uint32_t v = 0;
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+          const int p = 32 * half + 31 - 4 * j - q;
+          v |= (uint32_t)((blk[p >> 3] >> (8 * (p & 7))) & 0xff) << (8 * q);
+        }
+        s[j] = v;
+      }
+      s[7] &= 0x1fffffffu;
+      if (sc_is_canonical(s)) return;
+    }
+  }
+}
+
+// Scalar.Pick(blake2xb.New(seed)): the same draws from the root of the seed.  It keeps its own copy of the loop: written as
+// blake2xb_root + sc_pick_root, the PVSS challenge kernels compiled for sm_90a (CUDA 12.9) produced different challenges on
+// an H100, while the host build and a standalone kernel of the same code agreed with the reference.
 B2K_D void sc_pick(uint32_t* s, const uint8_t* seed, uint32_t len) {
   uint64_t h0[8], blk[8];
   blake2xb_root(h0, seed, len);
@@ -120,7 +182,7 @@ B2K_D void sc_pick(uint32_t* s, const uint8_t* seed, uint32_t len) {
     blake2xb_block(blk, h0, i);
     for (int half = 0; half < 2; half++) {
 #pragma unroll
-      for (int j = 0; j < 8; j++) {                     // limb j holds draw bytes 31 - 4 j - q (q = 0..3) at bits 8 q
+      for (int j = 0; j < 8; j++) {
         uint32_t v = 0;
 #pragma unroll
         for (int q = 0; q < 4; q++) {

@@ -78,11 +78,9 @@ B2K_D bool ed_eq_aff(const EdAff& a, const EdExt& Q) {
   return ed_eq_z1(p, Q);
 }
 
-// Q = geScalarMult(r, P) for a raw 256-bit r: signed 4-bit double-and-add over the cached table 1..8 P; a digit above 8 (only
-// the top one can be) selects nothing, as selectCached does
-B2K_D void ed_mul_var(EdExt& Q, const uint32_t* r, const EdExt& P) {
-  EdCached tp[8];
-  ed_cached_table(tp, P);
+// Q = geScalarMult(r, P) for a raw 256-bit r: signed 4-bit double-and-add over the cached table tp = 1..8 P; a digit above 8
+// (only the top one can be) selects nothing, as selectCached does
+B2K_D void ed_mul_cached(EdExt& Q, const uint32_t* r, const EdCached* tp) {
   int8_t e[64];
   sc_recode4(e, r);
   ed_set_identity(Q);
@@ -94,6 +92,12 @@ B2K_D void ed_mul_var(EdExt& Q, const uint32_t* r, const EdExt& P) {
       ed_add_cached(Q, Q, t.ypx, t.ymx, &t.z2, t.t2d, d < 0);
     }
   }
+}
+
+B2K_D void ed_mul_var(EdExt& Q, const uint32_t* r, const EdExt& P) {
+  EdCached tp[8];
+  ed_cached_table(tp, P);
+  ed_mul_cached(Q, r, tp);
 }
 
 // r = (-b) mod l, canonical, for any 256-bit b (Scalar.Neg)
