@@ -320,9 +320,9 @@ B2K_D void scalar_mul(Jac<typename CV::F>& r, const Scalar256& k, const Affine<t
 // ---- independent scalar multiplication, fixed signed windows (every curve) ---------------------------------------------
 // k P over signed radix-16 digits of the full 256-bit scalar and one affine table {P .. 8P}: 65 x (4 doublings + 1 mixed
 // addition), the same instruction stream in every lane (scalar_mul above pays an addition per bit as soon as ONE lane of
-// the warp has that bit set).  Valid for any k < 2^256 and any point of the curve: j P != infinity is only assumed for
-// j <= 8 when the table is normalised (true in the prime-order groups on this path; the exceptional cases of the additions
-// themselves are handled by jac_madd).
+// the warp has that bit set).  Valid for any k < 2^256 and any point of the curve: a table entry j P (j <= 8) that is
+// infinity -- BLS12-381 G1 has points of order 3, such as (0, +-2); the G2 twists and the bn254 / bn256 curves have no points of
+// order <= 8 -- is left out of the batched inversion and stored as the affine infinity (0, 0), which jac_madd adds as a no-op.
 template <class CV, class INV>
 B2K_D void scalar_mul_w4(Jac<typename CV::F>& r, const Scalar256& k, const Affine<typename CV::F>& p, INV inv_fn) {
   using F = typename CV::F;
@@ -336,9 +336,13 @@ B2K_D void scalar_mul_w4(Jac<typename CV::F>& r, const Scalar256& k, const Affin
     for (int j = 2; j < 8; j++) jac_madd(tj[j], tj[j - 1], p);
     F pre[8], acc, zi, zi2;
     f_set_one(acc);
-    for (int j = 1; j < 8; j++) { pre[j] = acc; f_mul(acc, acc, tj[j].Z); }
+    for (int j = 1; j < 8; j++) {
+      pre[j] = acc;
+      if (!jac_is_inf(tj[j])) f_mul(acc, acc, tj[j].Z);
+    }
     inv_fn(acc, acc);
     for (int j = 7; j >= 1; j--) {
+      if (jac_is_inf(tj[j])) { aff_set_inf(tab[j]); continue; }
       f_mul(zi, acc, pre[j]);
       f_mul(acc, acc, tj[j].Z);
       f_sqr(zi2, zi);

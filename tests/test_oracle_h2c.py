@@ -4,6 +4,8 @@ import hashlib
 import json
 import os
 
+import pytest
+
 from oracle import bls12381 as o
 from oracle import h2c_bls12381 as h
 
@@ -13,9 +15,20 @@ KAT = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "bls12381
 def test_expand_message_xmd_shape():
     out = h.expand_message_xmd(b"abc", b"QUUX-V01-CS02-with-expander-SHA256-128", 128)
     assert len(out) == 128 and out != bytes(128)
-    # RFC 9380 appendix K.1 vector (msg "", len 0x20) [FROM MEMORY of the published vector]
-    v = h.expand_message_xmd(b"", b"QUUX-V01-CS02-with-expander-SHA256-128", 32)
-    assert v.hex() == "68a985b87eb6b46952128911f2a4412bbc302a9d759667f87f7a21d803f07235"
+
+
+XMD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "xmd_sha256_vectors.json")))["vectors"]
+
+
+@pytest.mark.parametrize("dst_kind", ["short", "oversize"])
+def test_expand_message_xmd_rfc9380_vectors(dst_kind):
+    """RFC 9380 appendix K.1 (tests/golden/make_golden_xmd.py): five messages, 32 and 128 output bytes; the 256-byte DST takes
+    the H2C-OVERSIZE-DST- pre-hash of section 5.3.3 (the device refuses DSTs over 255 bytes, so only the oracle sees it)"""
+    vs = [v for v in XMD if (len(v["dst"]) > 255) == (dst_kind == "oversize")]
+    assert len(vs) == 10
+    for v in vs:
+        got = h.expand_message_xmd(v["msg"].encode(), v["dst"].encode(), v["len_in_bytes"])
+        assert got.hex() == v["uniform_bytes"], (len(v["msg"]), len(v["dst"]), v["len_in_bytes"])
 
 
 def test_isogeny_is_a_homomorphism_onto_the_curve():
