@@ -610,6 +610,34 @@ int b2k_ed25519_anon_verify(b2k_ctx* ctx, size_t n, const uint8_t* ring /*[n][32
                             const uint32_t* offsets /*[m+1]*/, const uint8_t* sigs, uint8_t* status /*[m]*/,
                             uint8_t* tags /*[m][32] or NULL*/);
 
+/* ---- edwards25519 ECIES (encrypt/ecies, hash SHA-256) -------------------------------------------------------------------
+ * Byte for byte ecies.Encrypt / ecies.Decrypt (encrypt/ecies/ecies.go:23-112) on edwards25519 with sha256.New, the calls of
+ * the Pedersen DKG's Deals (share/dkg/pedersen/dkg.go:364-385) and ProcessDeals (:470-494).  A ciphertext is
+ * R (32) || AES-256-GCM(body) || tag (16); the AES key and the GCM nonce are HKDF-SHA256(dh.MarshalBinary(), salt nil,
+ * info nil)[0:32] and [32:44]; no AAD.  R and the public keys decode like FromBytes (non-canonical y and small-order points
+ * accepted, all-zero bytes are the point of order 4).  Scalars (priv, r) are 32 raw little-endian bytes read as
+ * geScalarMult / geScalarMultBase read them: no reduction mod l, and a top signed digit above 8 selects nothing (see
+ * b2k_ed25519_msm).  Constant time on the secrets (key, r, dh, the derived key, AES and GHASH state, plaintext): no
+ * data-dependent branch or address on the device.  One length per call; bad data is only a status, never a call error.
+ * B2K_ERR_ARG: a null pointer, n == 0, len out of range, or n len too large.  Blocking, host buffers, staged through the
+ * context's input arena, which is cleared before the call returns.
+ *   B2K_ECIES_POINT  R (decrypt) or the public key (encrypt) does not decode: "invalid Ed25519 curve point"
+ *   B2K_ECIES_AUTH   the GCM tag does not match: "cipher: message authentication failed"
+ * A reference ciphertext shorter than 48 bytes never reaches these calls: below 32 bytes it is "invalid ecies cipher"; from
+ * 32 to 47 bytes the caller decodes R first ("invalid Ed25519 curve point"), then GCM Open fails on the short body.
+ *   replaces: ecies.Decrypt / ecies.Encrypt called once per ciphertext */
+#define B2K_ECIES_OK    0
+#define B2K_ECIES_POINT 1
+#define B2K_ECIES_AUTH  2
+#define B2K_ECIES_MAX_LEN ((size_t)1 << 16)
+/* len = ciphertext body incl. tag, 16 <= len <= B2K_ECIES_MAX_LEN + 16; msg[i] zeroed unless OK */
+int b2k_ed25519_ecies_decrypt(b2k_ctx* ctx, const uint8_t* priv /*[32] LE*/, size_t n, size_t len,
+                              const uint8_t* ctxt /*[n][32 + len]*/, uint8_t* msg /*[n][len - 16]*/, uint8_t* status /*[n]*/);
+/* len = plaintext length, 0 <= len <= B2K_ECIES_MAX_LEN; ctxt[i] zeroed unless OK */
+int b2k_ed25519_ecies_encrypt(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][32]*/, const uint8_t* r /*[n][32] LE*/,
+                              size_t len, const uint8_t* msg /*[n][len]*/, uint8_t* ctxt /*[n][32 + len + 16]*/,
+                              uint8_t* status /*[n]*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

@@ -81,6 +81,8 @@ def load_library() -> C.CDLL:
     sigs["b2k_ed25519_shuffle_verify"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp])
     sigs["b2k_ed25519_shuffle_sequence_verifiable"] = (C.c_int, [vp, sz, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp])
     sigs["b2k_ed25519_anon_verify"] = (C.c_int, [vp, sz, vp, C.c_int, vp, sz, sz, vp, vp, vp, vp, vp])
+    sigs["b2k_ed25519_ecies_decrypt"] = (C.c_int, [vp, vp, sz, sz, vp, vp, vp])
+    sigs["b2k_ed25519_ecies_encrypt"] = (C.c_int, [vp, sz, vp, vp, sz, vp, vp, vp])
     sigs["b2k_bn254_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn256_pairing_check"] = (C.c_int, [vp, sz, vp, vp, vp, vp, vp])
     sigs["b2k_bn254_recover_commit"] = (C.c_int, [vp, sz, vp, vp, vp])
@@ -689,6 +691,31 @@ class Engine:
         self._check(self.lib.b2k_ed25519_anon_verify(self.h, n, bufs[0][0], int(linkable), bufs[1][0], len(sc), m,
                                                      *[b[0] for b in bufs[2:]]))
         return bytes(status), bytes(tags)
+
+    # -- encrypt/ecies on edwards25519 (SHA-256) --------------------------------------------------------
+    def ed25519_ecies_decrypt(self, priv: bytes, ctxts, length: int):
+        """n x ecies.Decrypt(edwards25519, priv, ctxts[i], sha256.New); every ciphertext is 32 + length bytes (length =
+        body + tag, >= 16) -> ([n] messages of length - 16 bytes, zero unless OK; n status bytes (B2K_ECIES_*: 0 OK, 1 POINT,
+        2 AUTH))"""
+        n = len(ctxts)
+        assert len(priv) == 32 and all(len(c) == 32 + length for c in ctxts)
+        msg, status = bytearray(max(n * (length - 16), 1)), bytearray(n)
+        bufs = [_buf(x) for x in (bytes(priv), b"".join(ctxts) or b"\x00", msg, status)]
+        self._check(self.lib.b2k_ed25519_ecies_decrypt(self.h, bufs[0][0], n, length, *[b[0] for b in bufs[1:]]))
+        w = length - 16
+        return [bytes(msg[w * i:w * i + w]) for i in range(n)], bytes(status)
+
+    def ed25519_ecies_encrypt(self, pubs, rs, msgs):
+        """n x ecies.Encrypt(edwards25519, pubs[i], msgs[i], sha256.New) with the ephemeral scalars rs[i] (32 bytes LE); all
+        messages of one length -> ([n] ciphertexts R || C || tag, zero unless OK; n status bytes (0 OK, 1 POINT))"""
+        n = len(msgs)
+        length = len(msgs[0]) if n else 0
+        assert len(pubs) == n and len(rs) == n and all(len(m) == length for m in msgs)
+        out, status = bytearray(max(n * (length + 48), 1)), bytearray(n)
+        bufs = [_buf(x) for x in (b"".join(pubs) or b"\x00", b"".join(rs) or b"\x00", b"".join(msgs) or b"\x00", out, status)]
+        self._check(self.lib.b2k_ed25519_ecies_encrypt(self.h, n, bufs[0][0], bufs[1][0], length, *[b[0] for b in bufs[2:]]))
+        w = length + 48
+        return [bytes(out[w * i:w * i + w]) for i in range(n)], bytes(status)
 
     def bn254_pair(self, g1: bytes, g2: bytes) -> bytes:
         n = len(g1) // 64

@@ -213,29 +213,6 @@ B2K_D void bn256_hash_to_g1(Affine<B256Fp>& out, const uint8_t* msg, uint32_t ms
 }
 
 // ---- bn256 HashG1: HKDF-SHA256 + Shallue-van de Woestijne ------------------------------------------------------------
-// HMAC-SHA256 with a key of at most 64 bytes (longer keys are hashed first, RFC 2104), message given as three fragments
-B2K_NI void hmac_sha256(uint8_t* out32, const uint8_t* key, uint32_t key_len, const uint8_t* m1, uint32_t n1, const uint8_t* m2,
-                        uint32_t n2, const uint8_t* m3, uint32_t n3) {
-  uint8_t k[64], kh[32], inner[32];
-  Sha256 s;
-  if (key_len > 64) {
-    sha256_init(s); sha256_update(s, key, key_len); sha256_final(s, kh);
-    key = kh; key_len = 32;
-  }
-  for (uint32_t i = 0; i < 64; i++) k[i] = (i < key_len ? key[i] : 0) ^ 0x36;
-  sha256_init(s);
-  sha256_update(s, k, 64);
-  if (n1) sha256_update(s, m1, n1);
-  if (n2) sha256_update(s, m2, n2);
-  if (n3) sha256_update(s, m3, n3);
-  sha256_final(s, inner);
-  for (uint32_t i = 0; i < 64; i++) k[i] ^= 0x36 ^ 0x5c;
-  sha256_init(s);
-  sha256_update(s, k, 64);
-  sha256_update(s, inner, 32);
-  sha256_final(s, out32);
-}
-
 // gfp.go:137-148 sign0: +1 when the canonical value is >= (p-1)/2, else -1
 B2K_D int bn256_sign0(const B256Fp& a_mont) {
   B256Fp x;

@@ -1,5 +1,5 @@
-// sha256.cuh -- SHA-256 (FIPS 180-4), streaming over byte fragments, per thread.  Used by hash-to-curve (h2c.cuh, bn_hash.cuh)
-// and by the PVSS challenges (pvss.cuh); kept apart so that the edwards25519 units do not pull in BLS12-381 code.
+// sha256.cuh -- SHA-256 (FIPS 180-4), streaming over byte fragments, per thread, and HMAC-SHA256 on it.  Used by hash-to-curve
+// (h2c.cuh, bn_hash.cuh), by the PVSS challenges (pvss.cuh) and by ECIES's HKDF (ecies.cuh); kept apart so that the edwards25519 units do not pull in BLS12-381 code.
 #pragma once
 #include "ptx.cuh"
 
@@ -82,6 +82,29 @@ B2K_D void sha256_final(Sha256& s, uint8_t* out32) {
     out32[4 * i] = (uint8_t)(s.h[i] >> 24); out32[4 * i + 1] = (uint8_t)(s.h[i] >> 16);
     out32[4 * i + 2] = (uint8_t)(s.h[i] >> 8); out32[4 * i + 3] = (uint8_t)s.h[i];
   }
+}
+
+// HMAC-SHA256 with a key of at most 64 bytes (longer keys are hashed first, RFC 2104), message given as three fragments
+B2K_NI void hmac_sha256(uint8_t* out32, const uint8_t* key, uint32_t key_len, const uint8_t* m1, uint32_t n1, const uint8_t* m2,
+                        uint32_t n2, const uint8_t* m3, uint32_t n3) {
+  uint8_t k[64], kh[32], inner[32];
+  Sha256 s;
+  if (key_len > 64) {
+    sha256_init(s); sha256_update(s, key, key_len); sha256_final(s, kh);
+    key = kh; key_len = 32;
+  }
+  for (uint32_t i = 0; i < 64; i++) k[i] = (i < key_len ? key[i] : 0) ^ 0x36;
+  sha256_init(s);
+  sha256_update(s, k, 64);
+  if (n1) sha256_update(s, m1, n1);
+  if (n2) sha256_update(s, m2, n2);
+  if (n3) sha256_update(s, m3, n3);
+  sha256_final(s, inner);
+  for (uint32_t i = 0; i < 64; i++) k[i] ^= 0x36 ^ 0x5c;
+  sha256_init(s);
+  sha256_update(s, k, 64);
+  sha256_update(s, inner, 32);
+  sha256_final(s, out32);
 }
 
 }  // namespace b2k
