@@ -91,9 +91,10 @@ func (P *Point) Sub(P1, P2 kyber.Point) kyber.Point   { P.p.Sub(un(P1), un(P2));
 func (P *Point) Neg(A kyber.Point) kyber.Point        { P.p.Neg(un(A)); return P }
 
 // Mul replaces point.Mul (group/edwards25519/point.go:235-258): s*A, or s*B for a nil A, on the device.
-// Scalars travel as their 32 little-endian bytes (scalar.go:187-189: raw, unreduced on UnmarshalBinary -- the kernel
-// multiplies by the full 256-bit integer, so torsion components behave like in geScalarMult); points as 32-byte
-// compressed encodings (ge.go:99-150).
+// Scalars travel as their 32 little-endian bytes (scalar.go:187-189: raw, unreduced on UnmarshalBinary). The kernel
+// reads them as geScalarMult does: 64 signed nibbles, a top nibble above 8 (only from 2^255 on) selecting nothing, with
+// no reduction mod l, so torsion components behave as in the reference. Points travel as 32-byte compressed encodings
+// (ge.go:99-150).
 func (P *Point) Mul(s kyber.Scalar, A kyber.Point) kyber.Point {
 	src := A
 	if src == nil {

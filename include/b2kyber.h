@@ -477,9 +477,11 @@ int b2k_set_pairing_variant(b2k_ctx* ctx, int variant);
 int b2k_set_pairing_coop(b2k_ctx* ctx, int max_n);
 
 /* ---- edwards25519 ---------------------------------------------------------------------------------------- */
-/* out[i] = scalars[i] * points[i] on edwards25519.  scalars: RAW 256-bit little-endian integers (the reference
- * does not reduce on UnmarshalBinary, group/edwards25519/scalar.go:226-233); points and results: 32-byte
- * compressed (ge.go:99-150; non-canonical y accepted).  A point that does not decode -> B2K_ERR_POINT
+/* out[i] = scalars[i] * points[i] on edwards25519, as geScalarMult computes it.  scalars: RAW 256-bit little-endian
+ * integers (the reference does not reduce on UnmarshalBinary, group/edwards25519/scalar.go:226-233), read as 64 signed
+ * nibbles; a top nibble e63 above 8 (possible only from 2^255 on) selects nothing, so the product is then
+ * (k - e63 2^252) P; below 2^255 it is k P.  Points and results: 32-byte compressed (ge.go:99-150; non-canonical y
+ * accepted).  A point that does not decode -> B2K_ERR_POINT
  * (its output zeroed).   replaces: point.Mul, group/edwards25519/point.go:235-258 (geScalarMult, ge.go:443-502)
  * in loops such as util/test/group.go:118-122. */
 int b2k_ed25519_mul_batch(b2k_ctx* ctx, size_t n, const uint8_t* scalars /*[n][32] LE*/,

@@ -13,7 +13,8 @@
 // The challenge comparison is Scalar.Equal (pvss_challenge_is): the raw bytes of C0 against the final c.  What is hashed is
 // the canonical encoding of every point, the tag included.
 #pragma once
-#include "shuffle.cuh"
+#include "ed25519.cuh"
+#include "blake2b.cuh"
 
 namespace b2k {
 
@@ -35,13 +36,6 @@ B2K_D void ed_comb_table_column(EdCached* tab, uint32_t k, const EdExt& P) {
   }
 }
 
-B2K_D void ed_comb_add(EdExt& Q, const EdCached* row, int d) {
-  if (d != 0 && d <= 8) {
-    const EdCached& t = row[(d < 0 ? -d : d) - 1];
-    ed_add_cached(Q, Q, t.ypx, t.ymx, &t.z2, t.t2d, d < 0);
-  }
-}
-
 // Q = geScalarMultBase(a) over table ta + the same over table tb for b (tb may be null): one joint pass, at most 128 table
 // additions and 4 doublings
 B2K_D void ed_comb(EdExt& Q, const uint32_t* a, const EdCached* ta, const uint32_t* b, const EdCached* tb) {
@@ -50,13 +44,13 @@ B2K_D void ed_comb(EdExt& Q, const uint32_t* a, const EdCached* ta, const uint32
   if (tb) sc_recode4(eb, b);
   ed_set_identity(Q);
   for (int i = 1; i < 64; i += 2) {
-    ed_comb_add(Q, ta + 8 * (i >> 1), ea[i]);
-    if (tb) ed_comb_add(Q, tb + 8 * (i >> 1), eb[i]);
+    ed_digit_add(Q, ta + 8 * (i >> 1), ea[i]);
+    if (tb) ed_digit_add(Q, tb + 8 * (i >> 1), eb[i]);
   }
   ed_dbl_xyz(Q, Q); ed_dbl_xyz(Q, Q); ed_dbl_xyz(Q, Q); ed_dbl(Q, Q);
   for (int i = 0; i < 64; i += 2) {
-    ed_comb_add(Q, ta + 8 * (i >> 1), ea[i]);
-    if (tb) ed_comb_add(Q, tb + 8 * (i >> 1), eb[i]);
+    ed_digit_add(Q, ta + 8 * (i >> 1), ea[i]);
+    if (tb) ed_digit_add(Q, tb + 8 * (i >> 1), eb[i]);
   }
 }
 
@@ -114,7 +108,7 @@ B2K_D void anon_ring_step(uint32_t* c, const uint32_t* s, const EdCached* tb, co
   if (th) {
     EdExt T;
     ed_comb(PH, s, th, nullptr, nullptr);
-    ed_mul_cached(T, c, tagtab);
+    ed_mul_digits(T, c, tagtab);
     ed_add(PH, PH, T);
     EFp zi, zg, zh;                                         // one inversion for both (Montgomery's trick)
     fp_mul(zi, PG.Z, PH.Z);

@@ -5,7 +5,7 @@
 // (linkable only, one thread); the comb tables of B and H; then per chunk of ANON_CHUNK ring positions the tables of the chunk's
 // keys and one thread per signature walking the chunk; last the comparison with C0.  Every signature visits the ring positions
 // in the same order, so all threads of a step read the same key's table.
-#include "msm_host.cuh"
+#include "host_call.cuh"
 #include "anon.cuh"
 using namespace b2k_host;
 
@@ -104,17 +104,6 @@ __global__ void __launch_bounds__(ANON_BS) k_anon_finish(uint32_t m, int linkabl
 
 }  // namespace b2k
 
-namespace {
-
-unsigned blocks_of(uint64_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
-
-int bad_arg(b2k_ctx* ctx, const char* why) {
-  if (ctx) ctx->err = why;
-  return B2K_ERR_ARG;
-}
-
-}  // namespace
-
 extern "C" {
 
 int b2k_ed25519_anon_verify(b2k_ctx* ctx, size_t n, const uint8_t* ring, int linkable, const uint8_t* scope, size_t scope_len,
@@ -154,8 +143,7 @@ int b2k_ed25519_anon_verify(b2k_ctx* ctx, size_t n, const uint8_t* ring, int lin
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
   uint8_t base[32];
-  base[0] = 0x58;                                           // the base point B: y = 4/5, x positive
-  for (int q = 1; q < 32; q++) base[q] = 0x66;
+  ed_base_bytes(base);
   rc = status_begin(ctx);
   if (rc) return rc;
   CK(cudaMemcpyAsync(d_sig, sigs, m * siglen, cudaMemcpyHostToDevice, st));

@@ -3,7 +3,7 @@
 //   b2k_ed25519_ecies_encrypt   ecies.Encrypt(edwards25519, pub_i, msg_i, sha256.New) with the caller's ephemeral r_i
 // Both calls stage their inputs in the context's input arena, and clear the staged bytes (keys, r, plaintexts, ciphertexts)
 // before they return, so that no secret outlives the call in device memory the context keeps.
-#include "msm_host.cuh"
+#include "host_call.cuh"
 #include "ecies.cuh"
 using namespace b2k_host;
 
@@ -43,13 +43,6 @@ __global__ void __launch_bounds__(ECIES_BS) k_ecies_encrypt(size_t n, uint32_t l
 }  // namespace b2k
 
 namespace {
-
-unsigned blocks_of(size_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
-
-int bad_arg(b2k_ctx* ctx, const char* why) {
-  if (ctx) ctx->err = why;
-  return B2K_ERR_ARG;
-}
 
 size_t up256(size_t v) { return (v + 255) & ~size_t(255); }
 

@@ -1,6 +1,6 @@
 // b2k_eddsa.cu -- C ABI entry points for batched Ed25519 signature verification: eddsa.VerifyWithChecks
 // (sign/eddsa/eddsa.go:149-229) for n signatures per call, one thread each (eddsa.cuh).
-#include "msm_host.cuh"
+#include "host_call.cuh"
 #include "eddsa.cuh"
 using namespace b2k_host;
 
@@ -26,7 +26,7 @@ int b2k_ed25519_verify_dev(b2k_ctx* ctx, size_t n, const void* d_pks, const void
                            const void* d_sigs, void* d_status) {
   if (!ctx || !d_pks || !d_msgs || !d_offsets || !d_sigs || !d_status || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  k_ed25519_verify<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(n, (const uint8_t*)d_pks, (const uint8_t*)d_msgs,
+  k_ed25519_verify<<<blocks_of(n, 128), 128, 0, ctx->stream>>>(n, (const uint8_t*)d_pks, (const uint8_t*)d_msgs,
                                                                        (const uint32_t*)d_offsets, (const uint8_t*)d_sigs,
                                                                        (uint8_t*)d_status);
   CK(cudaGetLastError());

@@ -2,7 +2,7 @@
 //   b2k_ed25519_dleq_verify / _dev         dleq.Proof.Verify, proof/dleq/dleq.go:161-172, for n proofs
 //   b2k_ed25519_pvss_verify_enc_shares     pvss.VerifyEncShareBatch, share/pvss/pvss.go:168-194, for m deals in one call
 //   b2k_ed25519_pvss_verify_dec_shares     pvss.VerifyDecShareBatch, pvss.go:281-299
-#include "msm_host.cuh"
+#include "host_call.cuh"
 #include "pvss.cuh"
 using namespace b2k_host;
 
@@ -77,8 +77,6 @@ __global__ void __launch_bounds__(128) k_pvss_dec_verify(size_t n, const uint8_t
 
 namespace {
 
-unsigned blocks_of(size_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
-
 // copy the host inputs (pointer, bytes) into the device buffers, run enqueue(), copy the status bytes back and synchronise
 template <class Fn>
 int run_staged(b2k_ctx* ctx, std::initializer_list<std::pair<uint8_t*, std::pair<const uint8_t*, size_t>>> ins, Fn&& enqueue,
@@ -90,11 +88,6 @@ int run_staged(b2k_ctx* ctx, std::initializer_list<std::pair<uint8_t*, std::pair
   CK(cudaMemcpyAsync(status, d_status, n, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return B2K_OK;
-}
-
-int bad_arg(b2k_ctx* ctx) {
-  if (ctx) ctx->err = "bad argument";
-  return B2K_ERR_ARG;
 }
 
 int dleq_enqueue(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint8_t* h, const uint8_t* xg, const uint8_t* xh,
@@ -111,7 +104,7 @@ extern "C" {
 
 int b2k_ed25519_dleq_verify_dev(b2k_ctx* ctx, size_t n, const void* d_g, const void* d_h, const void* d_xg, const void* d_xh,
                                 const void* d_proofs, void* d_status) {
-  if (!ctx || !d_g || !d_h || !d_xg || !d_xh || !d_proofs || !d_status || n == 0) return bad_arg(ctx);
+  if (!ctx || !d_g || !d_h || !d_xg || !d_xh || !d_proofs || !d_status || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   return dleq_enqueue(ctx, n, (const uint8_t*)d_g, (const uint8_t*)d_h, (const uint8_t*)d_xg, (const uint8_t*)d_xh,
                       (const uint8_t*)d_proofs, (uint8_t*)d_status);
@@ -119,7 +112,7 @@ int b2k_ed25519_dleq_verify_dev(b2k_ctx* ctx, size_t n, const void* d_g, const v
 
 int b2k_ed25519_dleq_verify(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint8_t* h, const uint8_t* xg, const uint8_t* xh,
                             const uint8_t* proofs, uint8_t* status) {
-  if (!ctx || !g || !h || !xg || !xh || !proofs || !status || n == 0) return bad_arg(ctx);
+  if (!ctx || !g || !h || !xg || !xh || !proofs || !status || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   uint8_t *d_g = nullptr, *d_h = nullptr, *d_xg = nullptr, *d_xh = nullptr, *d_p = nullptr, *d_st = nullptr;
   int rc = arena_carve(ctx, [&](Carve& c) {
@@ -140,7 +133,7 @@ int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t 
                                        uint8_t* status) {
   if (!ctx || !h || !commits || !x || !sh || !v || !proofs || !status || m == 0 || t == 0 || n == 0 ||
       m * t >= (size_t(1) << 31) || m * n >= (size_t(1) << 31))
-    return bad_arg(ctx);
+    return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t mt = m * t, mn = m * n;
   uint8_t *d_h = nullptr, *d_c = nullptr, *d_x = nullptr, *d_sh = nullptr, *d_v = nullptr, *d_p = nullptr, *d_hashed = nullptr,
@@ -181,7 +174,7 @@ int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t 
 
 int b2k_ed25519_pvss_verify_dec_shares(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint8_t* x, const uint8_t* enc_v,
                                        const uint8_t* dec_v, const uint8_t* proofs, uint8_t* status) {
-  if (!ctx || !g || !x || !enc_v || !dec_v || !proofs || !status || n == 0) return bad_arg(ctx);
+  if (!ctx || !g || !x || !enc_v || !dec_v || !proofs || !status || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   uint8_t *d_g = nullptr, *d_x = nullptr, *d_e = nullptr, *d_d = nullptr, *d_p = nullptr, *d_st = nullptr;
   int rc = arena_carve(ctx, [&](Carve& c) {

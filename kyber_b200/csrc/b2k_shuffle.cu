@@ -5,7 +5,7 @@
 // Stages of the verifier, one kernel each (tools/perf_shuffle.py times them by name): decode every point once; U, W per shuffle;
 // one thread per thver; one thread per i for (33) and the Phi terms with a per-block sum; per shuffle the sum of the block
 // partials, (34), (35) and the status.  The transcript runs on host threads while the decode runs on the device.
-#include "msm_host.cuh"
+#include "host_call.cuh"
 #include "shuffle_transcript.h"
 using namespace b2k_host;
 
@@ -166,13 +166,6 @@ __global__ void __launch_bounds__(SHUF_BS) k_shuffle_seq_terms(uint32_t nq, uint
 
 namespace {
 
-unsigned blocks_of(uint64_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
-
-int bad_arg(b2k_ctx* ctx) {
-  if (ctx) ctx->err = "bad argument";
-  return B2K_ERR_ARG;
-}
-
 unsigned host_threads() {
   unsigned nt = std::thread::hardware_concurrency();
   return nt < 1 ? 1 : nt > 32 ? 32 : nt;
@@ -187,7 +180,7 @@ int b2k_ed25519_shuffle_verify(b2k_ctx* ctx, size_t m, size_t k, const uint8_t* 
                                const uint8_t* proto, uint32_t proto_len, uint8_t* status) {
   if (!ctx || !x || !y || !xbar || !ybar || !proofs || !status || (proto_len && !proto) || m == 0 || k < 2 ||
       m > B2K_SHUFFLE_MAX_PAIRS || k > B2K_SHUFFLE_MAX_PAIRS || m * k > B2K_SHUFFLE_MAX_PAIRS)
-    return bad_arg(ctx);
+    return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t nitem = 12 * k + 3, mk = m * k, nchunk = (k + SHUF_BS - 1) / SHUF_BS;
   uint8_t *d_p = nullptr, *d_in = nullptr, *d_g = nullptr, *d_h = nullptr, *d_zrho = nullptr, *d_tc = nullptr, *d_fl = nullptr,
@@ -249,7 +242,7 @@ int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, c
                                             uint8_t* y_up, uint8_t* x_down, uint8_t* y_down) {
   if (!ctx || !x || !y || !xbar || !ybar || !e || !x_up || !y_up || !x_down || !y_down || nq == 0 || k == 0 ||
       nq > B2K_SHUFFLE_MAX_PAIRS || k > B2K_SHUFFLE_MAX_PAIRS || nq * k > B2K_SHUFFLE_MAX_PAIRS)
-    return bad_arg(ctx);
+    return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t n = nq * k;
   uint8_t *d_in = nullptr, *d_e = nullptr, *d_out = nullptr;
@@ -262,7 +255,7 @@ int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, c
   });
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
+  if ((rc = status_begin(ctx))) return rc;
   const uint8_t* in[4] = {x, y, xbar, ybar};
   for (int q = 0; q < 4; q++) CK(cudaMemcpyAsync(d_in + q * n * 32, in[q], n * 32, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_e, e, nq * 32, cudaMemcpyHostToDevice, st));
@@ -272,9 +265,7 @@ int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, c
   ctx->launches += 2;
   uint8_t* outs[4] = {x_up, y_up, x_down, y_down};
   for (int q = 0; q < 4; q++) CK(cudaMemcpyAsync(outs[q], d_out + q * k * 32, k * 32, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(ctx->h_flags, ctx->d_flags, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return check_flags(ctx);
+  return status_finish(ctx);
 }
 
 }  // extern "C"

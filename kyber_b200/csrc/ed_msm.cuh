@@ -9,8 +9,8 @@
 // scan, partition and bin sort: msm_host.cuh, msm_sort.cuh) are shared, the point stages are written here:
 //   load       : decode (FromBytes, ge.go:110-150) into Niels form (y + x, y - x, 2 d x y), Montgomery, once per point; the scalar
 //                rule below; signed digits of 256-bit scalars (W = ceil(257 / c) windows) and the histogram
-//   accumulate : balanced slices of L sorted entries into extended (X:Y:Z:T) buckets by the mixed addition (7M, eddsa.cuh:
-//                ed_add_cached); -P swaps y + x with y - x and negates 2 d x y.  The addition law is complete, so identity,
+//   accumulate : balanced slices of L sorted entries into extended (X:Y:Z:T) buckets by the mixed addition (7M, ed25519.cuh:
+//                ed_madd); -P swaps y + x with y - x and negates 2 d x y.  The addition law is complete, so identity,
 //                doubling, negation and torsion operands take no branch, and the slices are skew-proof like the Weierstrass ones
 //   fix-up     : buckets cut by slice boundaries add their partials (ed_add); empty buckets are set to the identity here
 //   reduce     : one level of chunked running sums, a small multiple per chunk, a block-wide sum per window, Horner, encode
@@ -18,55 +18,12 @@
 // Scalars are read the way the reference's Point.Mul (geScalarMult, ge.go:443-502, varTime off) reads them: the plain
 // little-endian integer k, except that its signed-nibble recoding can leave a top digit e63 above 8, for which selectCached
 // (ge.go:419-433) selects nothing.  The product is then (k - e63 2^252) P, and the load pass multiplies by that integer instead
-// (ed_scalar_rule).  There is no reduction mod l: the points may have a torsion part.
+// (ed_scalar_rule, ed_scalar.cuh).  There is no reduction mod l: the points may have a torsion part.
 #pragma once
-#include "eddsa.cuh"
+#include "ed25519.cuh"
 #include "msm_sort.cuh"
 
 namespace b2k {
-
-// ---- scalars --------------------------------------------------------------------------------------------------------------
-// k -> the integer geScalarMult multiplies by, modulo the group exponent 8 l.  With low = k mod 2^252 and carry the carry the
-// recoding of the 63 lower nibbles leaves for the top one, e63 = (k >> 252) + carry.  Up to e63 = 8 that is k itself; above,
-// the top digit is dropped and the product is (low - carry 2^252) P, replaced here by low + carry (8 l - 2^252) < 2^256, which is
-// the same multiple of every point of the curve (8 l is the order of the whole group).
-B2K_D void ed_scalar_rule(uint32_t* k) {
-  int carry = 0;
-  for (int i = 0; i < 63; i++) {
-    const int v = (int)((k[i >> 3] >> (4 * (i & 7))) & 15u) + carry;
-    carry = (v + 8) >> 4;
-  }
-  if ((int)(k[7] >> 28) + carry <= 8) return;
-  k[7] &= 0x0fffffffu;
-  if (!carry) return;
-  uint32_t c[8];                                       // 8 l - 2^252 (l < 2^253: the shift stays in 256 bits)
-#pragma unroll
-  for (int j = 0; j < 8; j++) c[j] = (Ed25519Verify::ell(j) << 3) | (j ? Ed25519Verify::ell(j - 1) >> 29 : 0u);
-  c[7] -= 0x10000000u;
-  uint64_t s = 0;
-#pragma unroll
-  for (int j = 0; j < 8; j++) {
-    s += (uint64_t)k[j] + c[j];
-    k[j] = (uint32_t)s;
-    s >>= 32;
-  }
-}
-
-// ---- points ---------------------------------------------------------------------------------------------------------------
-B2K_D void ed_niels_identity(EdNiels& q) { fp_set_one(q.ypx); fp_set_one(q.ymx); fp_set_zero(q.t2d); }
-
-// FromBytes into Niels form; a point that does not decode becomes the identity and the call returns false
-B2K_D bool ed_load_niels(EdNiels& q, const uint8_t* b) {
-  EdExt p;
-  if (!ed_decode(p, b)) { ed_niels_identity(q); return false; }
-  EFp d2;
-  ed_load_const(d2, Ed25519Fp::ed_2d);
-  fp_add(q.ypx, p.Y, p.X); fp_sub(q.ymx, p.Y, p.X); fp_mul(q.t2d, p.T, d2);
-  return true;
-}
-
-// acc += q or acc -= q (mixed addition, 7M)
-B2K_D void ed_madd(EdExt& acc, const EdNiels& q, bool neg) { ed_add_cached(acc, acc, q.ypx, q.ymx, nullptr, q.t2d, neg); }
 
 // ---- load pass: point i to Niels form, scalar rule, digit columns and histogram (msm_digits_store) -------------------------------
 B2K_D bool ed_msm_load(size_t n, size_t i, const uint8_t* scalars, const uint8_t* wire, EdNiels* pts, const MsmPlan& pl,
@@ -144,19 +101,6 @@ B2K_D void ed_fixup_strided(EdExt& acc, uint32_t tid, uint32_t nt, uint32_t j0, 
 }
 
 // ---- reduction ------------------------------------------------------------------------------------------------------------
-// r = k p for a small k, double-and-add from the top bit
-B2K_D void ed_mul_small(EdExt& r, const EdExt& p, uint32_t k) {
-  if (!k) { ed_set_identity(r); return; }
-  int top = 31;
-  while (!((k >> top) & 1u)) top--;
-  EdExt acc = p;
-  for (int b = top - 1; b >= 0; b--) {
-    ed_dbl(acc, acc);
-    if ((k >> b) & 1u) ed_add(acc, acc, p);
-  }
-  r = acc;
-}
-
 // chunk t of m consecutive buckets of one window (B[k] holds digit magnitude k + 1): out = sum_k (k + 1) B[t m + k]
 B2K_D void ed_reduce_chunk(EdExt& out, const EdExt* B, int t, int m) {
   EdExt run, acc;
@@ -188,48 +132,18 @@ B2K_D void ed_msm_horner(EdExt& out, const EdExt* wsum, int W, int c) {
 }
 
 // ---- share/poly -----------------------------------------------------------------------------------------------------------
-// v = sum_j x^j C_j (Horner, poly.go:343-346), x v by double-and-add over the bits of x below its top bit (x >= 1)
-B2K_D void ed_pubpoly_horner(EdExt& v, const EdNiels* cm, uint32_t t, uint64_t x) {
-  int top = 63;
-  while (top > 0 && !((x >> top) & 1u)) top--;
-  ed_set_identity(v);
-  for (int j = (int)t - 1; j >= 0; j--) {
-    EdExt acc = v;
-    for (int b = top - 1; b >= 0; b--) {
-      ed_dbl(acc, acc);
-      if ((x >> b) & 1u) ed_add(acc, acc, v);
-    }
-    const EdNiels c = cm[j];
-    ed_add_cached(v, acc, c.ypx, c.ymx, nullptr, c.t2d, false);
-  }
-}
-
-// r = k B by geScalarMult's own schedule (ge.go:443-502): 64 signed nibbles (sc_recode4), a top digit above 8 selects nothing
-// (selectCached), four doublings per nibble; btab = 1..8 B (ed_load_base_table)
-B2K_D void ed_ge_scalar_mult_base(EdExt& r, const uint32_t* k, const EdNiels* btab) {
-  int8_t e[64];
-  sc_recode4(e, k);
-  ed_set_identity(r);
-  for (int i = 63; i >= 0; i--) {
-    if (i != 63) { ed_dbl_xyz(r, r); ed_dbl_xyz(r, r); ed_dbl_xyz(r, r); ed_dbl(r, r); }
-    const int d = e[i];
-    if (d != 0 && d <= 8) ed_madd(r, btab[(d < 0 ? -d : d) - 1], d < 0);
-  }
-}
+// r = k B by geScalarMult's schedule (ed_mul_digits) over btab = 1..8 B (ed_load_base_table)
+B2K_D void ed_ge_scalar_mult_base(EdExt& r, const uint32_t* k, const EdNiels* btab) { ed_mul_digits(r, k, btab); }
 
 // PubPoly.Check of one private share (index, 32-byte little-endian value) against t commitments in Niels form: the Horner value
-// and share B compared projectively (X1 Z2 = X2 Z1, Y1 Z2 = Y2 Z1)
+// and share B compared projectively
 B2K_D bool ed_pubpoly_check_one(const EdNiels* cm, uint32_t t, uint32_t index, const uint8_t* share, const EdNiels* btab) {
   EdExt v, w;
   ed_pubpoly_horner(v, cm, t, (uint64_t)index + 1u);
   uint32_t k[8];
   sc_load_le(k, share);
   ed_ge_scalar_mult_base(w, k, btab);
-  EFp a, b;
-  fp_mul(a, v.X, w.Z); fp_mul(b, w.X, v.Z);
-  if (!fp_eq(a, b)) return false;
-  fp_mul(a, v.Y, w.Z); fp_mul(b, w.Y, v.Z);
-  return fp_eq(a, b);
+  return ed_eq(v, w);
 }
 
 }  // namespace b2k

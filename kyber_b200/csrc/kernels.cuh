@@ -4,11 +4,9 @@
 #include "fp_inv.cuh"
 #include "msm_affine.cuh"
 #include "msm_sort.cuh"
+#include "host_call.cuh"                            // FLAG_*: the bits of the device status word
 
 namespace b2k {
-
-// error flag bits written by kernels
-enum : uint32_t { FLAG_SCALAR_RANGE = 1u, FLAG_POINT = 2u, FLAG_COMM_TIMEOUT = 32u };   // (4u: duplicate share index, b2k_share.cu)
 
 // ---- operand conversion: wire bytes -> Montgomery affine (AoS, one point = 2*N limbs) -----------
 template <class CV>

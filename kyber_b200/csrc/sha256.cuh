@@ -1,6 +1,7 @@
 // sha256.cuh -- SHA-256 (FIPS 180-4), streaming over byte fragments, per thread, and HMAC-SHA256 on it.  Used by hash-to-curve
-// (h2c.cuh, bn_hash.cuh), by the PVSS challenges (pvss.cuh) and by ECIES's HKDF (ecies.cuh); kept apart so that the edwards25519 units do not pull in BLS12-381 code.
+// (h2c.cuh, bn_hash.cuh), by the PVSS challenges (pvss.cuh, sha256_blocks) and by ECIES's HKDF (ecies.cuh); kept apart so that the edwards25519 units do not pull in BLS12-381 code.
 #pragma once
+#include <stddef.h>
 #include "ptx.cuh"
 
 namespace b2k {
@@ -82,6 +83,15 @@ B2K_D void sha256_final(Sha256& s, uint8_t* out32) {
     out32[4 * i] = (uint8_t)(s.h[i] >> 24); out32[4 * i + 1] = (uint8_t)(s.h[i] >> 16);
     out32[4 * i + 2] = (uint8_t)(s.h[i] >> 8); out32[4 * i + 3] = (uint8_t)s.h[i];
   }
+}
+
+// SHA-256 of nblk whole 64-byte blocks at p; digest (big-endian bytes) in out
+B2K_D void sha256_blocks(uint8_t* out, const uint8_t* p, size_t nblk) {
+  Sha256 s;
+  sha256_init(s);
+  for (size_t k = 0; k < nblk; k++) sha256_compress(s.h, p + 64 * k);
+  s.total = 64 * nblk;
+  sha256_final(s, out);
 }
 
 // HMAC-SHA256 with a key of at most 64 bytes (longer keys are hashed first, RFC 2104), message given as three fragments

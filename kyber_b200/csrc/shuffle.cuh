@@ -13,7 +13,7 @@
 // G or H absent means the base point: geScalarMultBase drops a top digit above 8 exactly as geScalarMult does, so the base is
 // just another variable base here.
 #pragma once
-#include "pvss.cuh"
+#include "ed25519.cuh"
 
 namespace b2k {
 
@@ -41,83 +41,6 @@ struct ShufItems {
   B2K_HD static uint64_t zalpha(uint64_t k, uint64_t i) { return 10 * k + 4 + i; }
   B2K_HD static bool is_point(uint64_t k, uint64_t j) { return !(j >= 5 * k + 3 && j < 6 * k + 4) && j < 10 * k + 4; }
 };
-
-// a decoded point (Z = 1); an operand that does not decode is stored as the identity and flags its shuffle
-struct EdAff { EFp x, y; };
-
-B2K_D void ed_from_aff(EdExt& p, const EdAff& a) { p.X = a.x; p.Y = a.y; fp_set_one(p.Z); fp_mul(p.T, a.x, a.y); }
-
-B2K_D bool ed_decode_aff(EdAff& a, const uint8_t* b) {
-  EdExt p;
-  const bool ok = ed_decode(p, b);
-  if (!ok) ed_set_identity(p);
-  a.x = p.X; a.y = p.Y;
-  return ok;
-}
-
-// the encoding of the base point B (y = 4/5, x positive)
-B2K_D void ed_base_bytes(uint8_t* b) {
-  b[0] = 0x58;
-  for (int j = 1; j < 32; j++) b[j] = 0x66;
-}
-
-B2K_D void ed_neg(EdExt& p) { fp_neg(p.X, p.X); fp_neg(p.T, p.T); }
-
-// exact equality of two projective points: X1 Z2 = X2 Z1 and Y1 Z2 = Y2 Z1
-B2K_D bool ed_eq(const EdExt& p, const EdExt& q) {
-  EFp a, b;
-  fp_mul(a, p.X, q.Z); fp_mul(b, q.X, p.Z);
-  if (!fp_eq(a, b)) return false;
-  fp_mul(a, p.Y, q.Z); fp_mul(b, q.Y, p.Z);
-  return fp_eq(a, b);
-}
-
-B2K_D bool ed_eq_aff(const EdAff& a, const EdExt& Q) {
-  EdExt p;
-  p.X = a.x; p.Y = a.y;
-  return ed_eq_z1(p, Q);
-}
-
-// Q = geScalarMult(r, P) for a raw 256-bit r: signed 4-bit double-and-add over the cached table tp = 1..8 P; a digit above 8
-// (only the top one can be) selects nothing, as selectCached does
-B2K_D void ed_mul_cached(EdExt& Q, const uint32_t* r, const EdCached* tp) {
-  int8_t e[64];
-  sc_recode4(e, r);
-  ed_set_identity(Q);
-  for (int i = 63; i >= 0; i--) {
-    if (i != 63) { ed_dbl_xyz(Q, Q); ed_dbl_xyz(Q, Q); ed_dbl_xyz(Q, Q); ed_dbl(Q, Q); }
-    const int d = e[i];
-    if (d != 0 && d <= 8) {
-      const EdCached& t = tp[(d < 0 ? -d : d) - 1];
-      ed_add_cached(Q, Q, t.ypx, t.ymx, &t.z2, t.t2d, d < 0);
-    }
-  }
-}
-
-B2K_D void ed_mul_var(EdExt& Q, const uint32_t* r, const EdExt& P) {
-  EdCached tp[8];
-  ed_cached_table(tp, P);
-  ed_mul_cached(Q, r, tp);
-}
-
-// r = (-b) mod l, canonical, for any 256-bit b (Scalar.Neg)
-B2K_D void sc_neg_mod_l(uint32_t* r, const uint32_t* b) {
-  uint32_t x[16];
-#pragma unroll
-  for (int j = 0; j < 8; j++) { x[j] = b[j]; x[j + 8] = 0; }
-  sc_reduce512(r, x);
-  uint32_t o = 0;
-#pragma unroll
-  for (int j = 0; j < 8; j++) o |= r[j];
-  if (!o) return;
-  uint64_t borrow = 0;
-#pragma unroll
-  for (int j = 0; j < 8; j++) {
-    const uint64_t d = (uint64_t)Ed25519Verify::ell(j) - r[j] - borrow;
-    r[j] = (uint32_t)d;
-    borrow = (d >> 63) & 1;
-  }
-}
 
 // thver(A, B, T, a, b): a A + Neg(b) B == T, a raw, b negated mod l, T decoded
 B2K_D bool shuffle_thver(const EdExt& A, const EdExt& B, const EdAff& T, const uint32_t* a, const uint32_t* b) {

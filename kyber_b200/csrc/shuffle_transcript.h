@@ -10,13 +10,14 @@
 // (unused, but it consumes stream); absorb ega5 || ssa0 in one write, pick t; absorb ssa2, pick c.  ssa4 is never absorbed.
 // Each absorb is one sequential BLAKE2b chain (hash.go keeps it so); the Zrho squeeze is spread over threads: every BLAKE2X
 // output block is independent, so blocks are hashed in parallel and a scan over the accept flags gives the positions.
-// BLAKE2b itself is pvss.cuh's (host-callable).
+// BLAKE2b itself is blake2b.cuh's (host-callable).
 #pragma once
 #include <cmath>
 #include <cstring>
 #include <thread>
 #include <vector>
 
+#include "blake2b.cuh"
 #include "shuffle.cuh"
 
 namespace b2k {
@@ -26,7 +27,7 @@ namespace shuffle_host {
 constexpr uint8_t kL[32] = {0xed, 0xd3, 0xf5, 0x5c, 0x1a, 0x63, 0x12, 0x58, 0xd6, 0x9c, 0xf7, 0xa2, 0xde, 0xf9, 0xde, 0x14,
                             0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0,    0x10};
 
-// BLAKE2b-512 streamed from memory (the compression of pvss.cuh)
+// BLAKE2b-512 streamed from memory (the compression of blake2b.cuh)
 struct Blake2bStream {
   uint64_t* h;
   uint64_t t = 0;

@@ -5,13 +5,14 @@ oracle/ed25519.py.
   Encrypt(P, r, msg) = R || AES-GCM_k(nonce, msg),  R = r B, dh = r P, k || nonce = HKDF(dh.MarshalBinary(), nil, nil)[0:44]
   Decrypt(priv, ct)  = GCM Open under HKDF(priv R) of ct[32:], R = FromBytes(ct[:32])
 
-Scalars are the raw 32 little-endian bytes, multiplied as geScalarMult / geScalarMultBase multiply them: the plain integer,
-except that a top signed digit e63 above 8 selects nothing (the product is then (k - e63 2^252) P).  TEST INFRASTRUCTURE."""
+Scalars are the raw 32 little-endian bytes, multiplied as geScalarMult / geScalarMultBase multiply them (ed25519.point_mul: the
+plain integer, except that a top signed digit e63 above 8 selects nothing).  TEST INFRASTRUCTURE."""
 from __future__ import annotations
 import hashlib
 import hmac
 
 from . import ed25519 as ed
+from .ed25519 import effective_scalar, top_digit          # noqa: F401 (the digit rule, shared with Point.Mul)
 
 OK, POINT, AUTH = 0, 1, 2               # B2K_ECIES_* of include/b2kyber.h
 MAX_LEN = 1 << 16
@@ -134,25 +135,9 @@ def hkdf_sha256(secret: bytes, length: int, salt: bytes = None, info: bytes = b"
 
 
 # ---- ECIES -------------------------------------------------------------------------------------------------------------------
-def top_digit(k: int) -> int:
-    """e63 of the signed-nibble recoding (ge.go:443-466): the top nibble plus the carry out of the lower 63"""
-    carry = 0
-    for i in range(63):
-        v = ((k >> (4 * i)) & 15) + carry
-        carry = (v + 8) >> 4
-    return (k >> 252) + carry
-
-
-def effective_scalar(scalar_le: bytes) -> int:
-    """the integer geScalarMult and geScalarMultBase multiply by"""
-    k = int.from_bytes(scalar_le, "little")
-    e63 = top_digit(k)
-    return k - (e63 << 252) if e63 > 8 else k
-
-
 def mul(scalar_le: bytes, point=None) -> bytes:
     """Point.Mul(s, P).MarshalBinary() for a decoded point (None = the base point)"""
-    return ed.encode(ed.scalar_mult(effective_scalar(scalar_le) % (8 * ed.L), ed.BASE if point is None else point))
+    return ed.point_mul(scalar_le, None if point is None else ed.encode(point))
 
 
 def derive(dh: bytes):

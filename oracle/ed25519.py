@@ -2,7 +2,8 @@
 
 Restates, from the in-tree reference (group/edwards25519 is a ref10 port; the group law fixes the result):
   point.Mul             group/edwards25519/point.go:235-258  (nil base -> B; raw 256-bit little-endian scalar,
-                        no reduction on UnmarshalBinary: scalar.go:226-233)
+                        no reduction on UnmarshalBinary: scalar.go:226-233, read as geScalarMult's signed
+                        nibbles: a top digit above 8 selects nothing -> effective_scalar)
   geScalarMult / Base / Vartime   ge.go:443-502, :373-417, ge_mult_vartime.go:11-73 -> scalar_mult()
   ToBytes / FromBytes   ge.go:99-107, :110-150 (y little-endian, sign(x) in bit 255; non-canonical y accepted)
   Scalar.Pick           scalar.go:180-185 -> random.Int(l) util/random/rand.go:19-46 (mask to bitlen, big-endian,
@@ -91,9 +92,25 @@ def decode(b: bytes):
     return (x, y)
 
 
+_K63 = sum(8 << (4 * i) for i in range(63))
+
+
+def top_digit(k: int) -> int:
+    """e63 of geScalarMult's signed-nibble recoding (ge.go:443-466), in closed form: the carry pass over the 63 lower nibbles
+    is the sum low + 0x88..8 (63 nibbles), its carry into the top nibble bit 252 of that sum"""
+    return (k >> 252) + (((k & ((1 << 252) - 1)) + _K63) >> 252)
+
+
+def effective_scalar(k: int) -> int:
+    """the integer geScalarMult (and geScalarMultBase) multiplies by, modulo 8 l, the order of the whole group: k itself up to a
+    top digit of 8 (every k below 2^255), else k - e63 2^252, because selectCached (ge.go:419-433) selects nothing for it"""
+    e63 = top_digit(k)
+    return k if e63 <= 8 else (k - (e63 << 252)) % (8 * L)
+
+
 def point_mul(scalar_le: bytes, point32: bytes | None) -> bytes:
     """point.Mul(s, P).MarshalBinary(): s is the raw little-endian 32-byte scalar, point32 = None means base."""
-    k = int.from_bytes(scalar_le, "little")
+    k = effective_scalar(int.from_bytes(scalar_le, "little"))
     pt = BASE if point32 is None else decode(point32)
     if pt is None:
         raise ValueError("invalid point")

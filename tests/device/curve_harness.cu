@@ -1,5 +1,5 @@
 // curve_harness.cu -- test-only entry points into the per-thread curve code (ec.cuh, curves.cuh, codec.cuh, msm.cuh, h2c.cuh,
-// h2c_g2.cuh, ed25519.cuh, eddsa.cuh, ed_msm.cuh, shuffle.cuh), one case per thread on RAW MONTGOMERY LIMBS, so that a test picks
+// h2c_g2.cuh, ed25519.cuh), one case per thread on RAW MONTGOMERY LIMBS, so that a test picks
 // the coordinates, the projective scale and the exceptional operands itself.  Not a library unit: the library headers are
 // included unchanged.  Built three times by __graft_entry__.build() with the library's NVCC_FLAGS, like field_harness.cu:
 //   libcurve_harness_compact.so   -DB2K_COMPACT_FIELD=1
@@ -23,7 +23,7 @@
 #include "../../kyber_b200/csrc/bn_pairing.cuh"
 #include "../../kyber_b200/csrc/msm.cuh"
 #include "../../kyber_b200/csrc/msm_affine.cuh"
-#include "../../kyber_b200/csrc/shuffle.cuh"
+#include "../../kyber_b200/csrc/ed25519.cuh"
 #include <stddef.h>
 #include <utility>
 #ifdef __CUDACC__

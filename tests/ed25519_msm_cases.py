@@ -3,14 +3,15 @@
 ge_scalar_mult restates the reference's default Point.Mul (group/edwards25519/ge.go:443-502, geScalarMult, varTime off)
 literally: 4-bit nibbles of the 32 scalar bytes, the carry pass that makes them signed, the cached table 1..8 A, selectCached
 (ge.go:419-433), which selects NOTHING for a digit above 8, and four doublings per nibble.  Below 2^255 it is the plain
-product k A; from 2^255 on, a top digit e63 = (k >> 252) + carry above 8 is dropped.  effective_scalar gives the integer the
-device multiplies by instead (modulo 8 l, the order of the whole group), so that expected sums of many terms stay one
-multiplication of the base point."""
+product k A; from 2^255 on, a top digit e63 = (k >> 252) + carry above 8 is dropped.  The oracle's effective_scalar gives the
+integer the device multiplies by instead (modulo 8 l, the order of the whole group), so that expected sums of many terms stay
+one multiplication of the base point; ge_scalar_mult pins it."""
 from __future__ import annotations
 
 import random
 
 from oracle import ed25519 as ed
+from oracle.ed25519 import effective_scalar, top_digit          # noqa: F401 (the rule the cases are built on)
 
 P, L = ed.P, ed.L
 IDENTITY = ed.encode(ed.IDENT)          # 01 00 .. 00
@@ -68,26 +69,6 @@ def ge_scalar_mult(k_bytes: bytes, point):
             t = ed._ext_add(t, t)
         t = ed._ext_add(t, select(e[i]))
     return _affine(t)
-
-
-def top_digit(k: int) -> int:
-    return nibbles(k.to_bytes(32, "little"))[63]
-
-
-_K63 = sum(8 << (4 * i) for i in range(63))
-
-
-def top_digit_fast(k: int) -> int:
-    """e63 in closed form: the carry pass is the recoding low + 0x88..8 (63 nibbles), its carry the bit 252 of that sum"""
-    return (k >> 252) + (((k & ((1 << 252) - 1)) + _K63) >> 252)
-
-
-def effective_scalar(k: int) -> int:
-    """the integer geScalarMult multiplies by, modulo 8 l: k itself up to a top digit of 8, else k - e63 2^252"""
-    if k < 1 << 255:
-        return k
-    e63 = top_digit_fast(k)
-    return k if e63 <= 8 else (k - (e63 << 252)) % (8 * L)
 
 
 def crafted_high_scalars(rng: random.Random):

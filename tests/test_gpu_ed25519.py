@@ -1,9 +1,12 @@
 """GPU parity: edwards25519 batch Point.Mul through the C ABI vs the oracle, which is pinned by the reference's
 seeded KAT (examples/dh_test.go:17-49).  BASELINE configs[0]: batch of 1024 Point.Mul (seed b2k/c1)."""
+import random
+
 import pytest
 
 from kyber_b200 import B2KError, workload as wl
 from oracle import ed25519 as ed
+import ed25519_msm_cases as mc
 
 pytestmark = pytest.mark.gpu
 
@@ -41,6 +44,13 @@ def test_raw_scalars_torsion_and_bad_points(engine):
     out = engine.ed25519_mul_batch(b"".join(k.to_bytes(32, "little") for k in ks), b"".join(pts))
     for i, (k, p) in enumerate(zip(ks, pts)):
         assert out[32 * i:32 * i + 32] == ed.point_mul(k.to_bytes(32, "little"), p), i
+    high = mc.crafted_high_scalars(random.Random(6))            # geScalarMult's rule: e63 = 8 kept, 9 and 16 dropped
+    assert {mc.top_digit(k) for k in high} >= {8, 9, 16}
+    ks = high * 2
+    pts = [ed.encode(ed.BASE)] * len(high) + [mixed] * len(high)
+    out = engine.ed25519_mul_batch(b"".join(k.to_bytes(32, "little") for k in ks), b"".join(pts))
+    for i, (k, p) in enumerate(zip(ks, pts)):
+        assert out[32 * i:32 * i + 32] == ed.point_mul(k.to_bytes(32, "little"), p), (i, hex(k))
     with pytest.raises(B2KError) as e:
         engine.ed25519_mul_batch((1).to_bytes(32, "little"), (2).to_bytes(32, "little"))     # y = 2 is not on the curve
     assert e.value.code == -5

@@ -308,10 +308,13 @@ def test_bn254_pairing_bodies():
 
 def test_ed25519_and_inversion_bodies():
     from oracle import ed25519 as ed
+    import ed25519_msm_cases as mc
     lib = _lib("emul_ed")
     t8 = bytes.fromhex("c7176a703d4dd84fba3c0b760d10670f2a2053fa2c39ccc64ec7fd7792ac037a")
+    high = mc.crafted_high_scalars(random.Random(5))            # geScalarMult's rule: e63 = 8 kept, 9 and 16 dropped
+    assert {mc.top_digit(k) for k in high} >= {8, 9, 16}
     for pt in (ed.encode(ed.BASE), t8, ed.encode(ed.add(ed.scalar_mult(77), ed.decode(t8)))):
-        for k in (0, 1, ed.L, ed.L + 5, (1 << 255) - 1, 0x1234567890ABCDEF):
+        for k in [0, 1, ed.L, ed.L + 5, (1 << 255) - 1, 0x1234567890ABCDEF] + high:
             out = ctypes.create_string_buffer(32)
             assert lib.emul_ed25519_mul(k.to_bytes(32, "little"), pt, out) == 1
             assert out.raw == ed.point_mul(k.to_bytes(32, "little"), pt)

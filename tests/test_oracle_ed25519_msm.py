@@ -55,7 +55,16 @@ def test_0x8f_with_and_without_a_carry_into_nibble_62():
 def test_closed_form_top_digit_matches_the_carry_pass():
     rng = random.Random(4)
     for k in cases.crafted_high_scalars(rng) + [rng.getrandbits(256) for _ in range(2000)] + [0, (1 << 256) - 1]:
-        assert cases.top_digit_fast(k) == cases.top_digit(k), hex(k)
+        assert cases.top_digit(k) == cases.nibbles(_b(k))[63], hex(k)
+
+
+def test_point_mul_is_ge_scalar_mult_on_both_sides_of_the_rule():
+    rng = random.Random(12)
+    ks = cases.crafted_high_scalars(rng)
+    assert {cases.top_digit(k) for k in ks} >= {8, 9, 16}
+    for k in ks:
+        for pt in (ed.BASE, ed.decode(cases.mixed_point(3))):
+            assert ed.point_mul(_b(k), ed.encode(pt)) == ed.encode(cases.ge_scalar_mult(_b(k), pt)), hex(k)
 
 
 def test_top_digit_8_is_kept():

@@ -1,5 +1,5 @@
 """GPU timing of the edwards25519 MSM (b2k_ed25519_msm_dev) with its stage split, next to the per-term alternative,
-b2k_ed25519_mul_batch_dev (one bit-serial Point.Mul per thread) on the same inputs, at n = 2^10, 2^16 and 2^20.
+b2k_ed25519_mul_batch_dev (one Point.Mul per thread, geScalarMult's signed-nibble double-and-add) on the same inputs, at n = 2^10, 2^16 and 2^20.
 Both are timed with CUDA events on the device-pointer forms after a warm-up; the card, its power limit and its maximum SM
 clock are read in the same run.
 Usage: python tools/perf_ed25519_msm.py --out DIR   (writes DIR/perf_ed25519_msm.txt and DIR/perf_ed25519_msm.jsonl)"""
