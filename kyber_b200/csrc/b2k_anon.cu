@@ -124,56 +124,48 @@ int b2k_ed25519_anon_verify(b2k_ctx* ctx, size_t n, const uint8_t* ring, int lin
   Blake2bMid* d_mid = nullptr;
   EdAff* d_taga = nullptr;
   EdCached *d_ftab = nullptr, *d_ktab = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_sig = c.take<uint8_t>(m * siglen);
-    d_msg = c.take<uint8_t>(mbytes ? mbytes : 1);
-    d_off = c.take<uint32_t>(m + 1);
-    d_scope = c.take<uint8_t>(slen ? slen : 1);
-    d_ring = c.take<uint8_t>(n ? 32 * n : 1);
+  uint8_t base[32];
+  ed_base_bytes(base);
+  return host_call(ctx, [&](Carve& c) {
+    d_sig = c.in(sigs, m, siglen);
+    d_msg = c.in(msgs, mbytes);
+    d_off = c.in(offsets, m + 1);
+    d_scope = c.in(scope, slen);
+    d_ring = c.in(ring, n, 32);
     d_fix = c.take<uint8_t>(64);
-    d_tagb = c.take<uint8_t>(32 * m);
-    d_st = c.take<uint8_t>(m);
-    d_tags = c.take<uint8_t>(32 * m);
-    d_c = c.take<uint32_t>(8 * m);
+    c.copy_in(d_fix, base, 32);
+    d_tagb = c.take<uint8_t>(m, 32);
+    d_st = c.out(status, m);
+    d_tags = c.take<uint8_t>(m, 32);
+    if (tags) c.copy_out(tags, d_tags, 32 * m);
+    d_c = c.take<uint32_t>(m, 8);
     d_mid = c.take<Blake2bMid>(m);
     d_taga = c.take<EdAff>(m);
     d_ftab = c.take<EdCached>(nfix * 8 * ANON_ROWS);
     d_ktab = c.take<EdCached>((kmax ? kmax : 1) * 8 * ANON_ROWS);
-  });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  uint8_t base[32];
-  ed_base_bytes(base);
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d_sig, sigs, m * siglen, cudaMemcpyHostToDevice, st));
-  if (mbytes) CK(cudaMemcpyAsync(d_msg, msgs, mbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_off, offsets, (m + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (slen) CK(cudaMemcpyAsync(d_scope, scope, slen, cudaMemcpyHostToDevice, st));
-  if (n) CK(cudaMemcpyAsync(d_ring, ring, 32 * n, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_fix, base, 32, cudaMemcpyHostToDevice, st));
-  const unsigned gm = blocks_of(m, ANON_BS);
-  k_anon_setup<<<gm, ANON_BS, 0, st>>>((uint32_t)m, (uint32_t)n, linkable, d_msg, d_off, d_sig, siglen, d_scope, (uint32_t)slen,
-                                       d_mid, d_c, d_taga, d_tagb, d_st);
-  int launches = 2;
-  if (n) {
-    if (linkable) { k_anon_link_base<<<1, 1, 0, st>>>(d_scope, (uint32_t)slen, d_fix, ctx->d_flags); launches++; }
-    k_anon_tables<<<blocks_of(8 * nfix, ANON_BS), ANON_BS, 0, st>>>((uint32_t)nfix, d_fix, d_ftab, ctx->d_flags);
-    launches++;
-    for (size_t i0 = 0; i0 < n; i0 += ANON_CHUNK) {
-      const uint32_t cnt = (uint32_t)(n - i0 < ANON_CHUNK ? n - i0 : ANON_CHUNK);
-      k_anon_tables<<<blocks_of(8 * cnt, ANON_BS), ANON_BS, 0, st>>>(cnt, d_ring + 32 * i0, d_ktab, ctx->d_flags);
-      k_anon_ring_step<<<gm, ANON_BS, 0, st>>>((uint32_t)m, (uint32_t)i0, cnt, linkable, d_sig, siglen, d_ftab, d_ktab, d_mid, d_c,
-                                               d_taga, d_st);
-      launches += 2;
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    const unsigned gm = blocks_of(m, ANON_BS);
+    k_anon_setup<<<gm, ANON_BS, 0, st>>>((uint32_t)m, (uint32_t)n, linkable, d_msg, d_off, d_sig, siglen, d_scope, (uint32_t)slen,
+                                         d_mid, d_c, d_taga, d_tagb, d_st);
+    int launches = 2;
+    if (n) {
+      if (linkable) { k_anon_link_base<<<1, 1, 0, st>>>(d_scope, (uint32_t)slen, d_fix, ctx->d_flags); launches++; }
+      k_anon_tables<<<blocks_of(8 * nfix, ANON_BS), ANON_BS, 0, st>>>((uint32_t)nfix, d_fix, d_ftab, ctx->d_flags);
+      launches++;
+      for (size_t i0 = 0; i0 < n; i0 += ANON_CHUNK) {
+        const uint32_t cnt = (uint32_t)(n - i0 < ANON_CHUNK ? n - i0 : ANON_CHUNK);
+        k_anon_tables<<<blocks_of(8 * cnt, ANON_BS), ANON_BS, 0, st>>>(cnt, d_ring + 32 * i0, d_ktab, ctx->d_flags);
+        k_anon_ring_step<<<gm, ANON_BS, 0, st>>>((uint32_t)m, (uint32_t)i0, cnt, linkable, d_sig, siglen, d_ftab, d_ktab, d_mid, d_c,
+                                                 d_taga, d_st);
+        launches += 2;
+      }
     }
-  }
-  k_anon_finish<<<gm, ANON_BS, 0, st>>>((uint32_t)m, linkable, d_sig, siglen, d_c, d_tagb, d_st, d_tags);
-  CK(cudaGetLastError());
-  ctx->launches += launches;
-  CK(cudaMemcpyAsync(status, d_st, m, cudaMemcpyDeviceToHost, st));
-  if (tags) CK(cudaMemcpyAsync(tags, d_tags, 32 * m, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+    k_anon_finish<<<gm, ANON_BS, 0, st>>>((uint32_t)m, linkable, d_sig, siglen, d_c, d_tagb, d_st, d_tags);
+    CK(cudaGetLastError());
+    ctx->launches += launches;
+    return B2K_OK;
+  });
 }
 
 }  // extern "C"

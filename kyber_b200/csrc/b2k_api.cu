@@ -44,23 +44,9 @@ T* arena_take_impl(b2k_ctx* ctx, size_t count) {
   return reinterpret_cast<T*>(a.base + off);
 }
 
-inline size_t pad256(size_t b) { return (b + 255) & ~size_t(255); }
-
 }  // namespace
 
 int b2k_arena_reserve(b2k_ctx* ctx, size_t bytes) { return arena_reserve_impl(ctx, bytes); }
-void* b2k_arena_in(b2k_ctx* ctx, size_t bytes) {
-  Arena& a = ctx->arena_in;
-  if (bytes <= a.cap) return a.base;
-  if (a.base) {
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess || cudaFree(a.base) != cudaSuccess) return nullptr;
-    a.base = nullptr; a.cap = 0;
-  }
-  const size_t want = bytes + (bytes >> 2) + 4096;
-  if (cudaMalloc(&a.base, want) != cudaSuccess) { a.base = nullptr; return nullptr; }
-  a.cap = want;
-  return a.base;
-}
 void* b2k_arena_take(b2k_ctx* ctx, size_t bytes) { return arena_take_impl<char>(ctx, bytes); }
 
 using namespace b2k_host;
@@ -103,7 +89,6 @@ void b2k_destroy(b2k_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->arena.base) cudaFree(ctx->arena.base);
-  if (ctx->arena_in.base) cudaFree(ctx->arena_in.base);
   if (ctx->pair_scratch) cudaFree(ctx->pair_scratch);
   if (ctx->d_flags) cudaFree(ctx->d_flags);
   if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
@@ -240,7 +225,12 @@ int b2k_set_msm_variant(b2k_ctx* ctx, int v1) {
 int b2k_bls12381_g1_msm(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return msm_host<Bls381G1>(c, n, s, p, o); }
 int b2k_bls12381_g1_msm_affine(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return msm_host<Bls381G1>(c, n, s, p, o, 1); }
 int b2k_bls12381_g1_msm_async(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return msm_host<Bls381G1>(c, n, s, p, o, 0, false); }
-int b2k_wait(b2k_ctx* c) { return msm_wait(c); }
+// also the status query of the *_dev entry points, which only enqueue: the device status word is sticky across them
+int b2k_wait(b2k_ctx* ctx) {
+  if (!ctx) return B2K_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  return status_finish(ctx);
+}
 int b2k_bls12381_g1_msm_dev(b2k_ctx* c, size_t n, const void* s, const void* p, void* o) {
   if (c && c->msm_layout == 1) return b2k_internal_bls12381_g1_msm_dev_inlined(c, n, s, p, o, 0);
   return msm_dev<Bls381G1>(c, n, s, p, o);

@@ -52,50 +52,45 @@ extern "C" {
 int b2k_bn254_pair(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* gt) {
   if (!ctx || !g1 || !g2 || !gt || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, n * (64 + 128 + 384) + 4096);
-  if (rc) return rc;
-  uint8_t* d1 = arena_take<uint8_t>(ctx, n * 64);
-  uint8_t* d2 = arena_take<uint8_t>(ctx, n * 128);
-  uint8_t* dg = arena_take<uint8_t>(ctx, n * 384);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(d1, g1, n * 64, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d2, g2, n * 128, cudaMemcpyHostToDevice, st));
-  if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 8192 ? ctx->coop_max_n : 8192))   // break-even measured near 8 192 on this curve
-    coop::k_coop_bn_pair<Coop254, Bn254Pair><<<(unsigned)n, 32, Coop254::L::BYTES, st>>>(n, d1, d2, dg, ctx->d_flags);
-  else
-    k_bn254_pair<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, d1, d2, dg, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(gt, dg, n * 384, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d1 = nullptr, *d2 = nullptr, *dg = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d1 = c.in(g1, n, 64);
+    d2 = c.in(g2, n, 128);
+    dg = c.out(gt, n, 384);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 8192 ? ctx->coop_max_n : 8192))   // break-even measured near 8 192 on this curve
+      coop::k_coop_bn_pair<Coop254, Bn254Pair><<<(unsigned)n, 32, Coop254::L::BYTES, st>>>(n, d1, d2, dg, ctx->d_flags);
+    else
+      k_bn254_pair<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, d1, d2, dg, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 int b2k_bn254_pairing_check(b2k_ctx* ctx, size_t n, const uint8_t* a1, const uint8_t* a2, const uint8_t* b1,
                             const uint8_t* b2, uint8_t* ok) {
   if (!ctx || !a1 || !a2 || !b1 || !b2 || !ok || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, n * (2 * 64 + 2 * 128 + 1) + 8192);
-  if (rc) return rc;
-  uint8_t* da1 = arena_take<uint8_t>(ctx, n * 64);
-  uint8_t* da2 = arena_take<uint8_t>(ctx, n * 128);
-  uint8_t* db1 = arena_take<uint8_t>(ctx, n * 64);
-  uint8_t* db2 = arena_take<uint8_t>(ctx, n * 128);
-  uint8_t* dok = arena_take<uint8_t>(ctx, n);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(da1, a1, n * 64, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(da2, a2, n * 128, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(db1, b1, n * 64, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(db2, b2, n * 128, cudaMemcpyHostToDevice, st));
-  if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 8192 ? ctx->coop_max_n : 8192))   // break-even measured near 8 192 on this curve
-    coop::k_coop_bn_pairing_check<Coop254><<<(unsigned)n, 32, Coop254::L::BYTES, st>>>(n, da1, da2, db1, db2, dok, ctx->d_flags);
-  else
-    k_bn254_pairing_check<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, da1, da2, db1, db2, dok, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(ok, dok, n, cudaMemcpyDeviceToHost, st));
-  { int rc2 = status_finish(ctx); return rc2 == B2K_ERR_POINT ? B2K_OK : rc2; }   // a malformed operand already failed its own check
+  uint8_t *da1 = nullptr, *da2 = nullptr, *db1 = nullptr, *db2 = nullptr, *dok = nullptr;
+  const int rc = host_call(ctx, [&](Carve& c) {
+    da1 = c.in(a1, n, 64);
+    da2 = c.in(a2, n, 128);
+    db1 = c.in(b1, n, 64);
+    db2 = c.in(b2, n, 128);
+    dok = c.out(ok, n);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    if (ctx->coop_max_n > 0 && n <= (size_t)(ctx->coop_max_n < 8192 ? ctx->coop_max_n : 8192))   // break-even measured near 8 192 on this curve
+      coop::k_coop_bn_pairing_check<Coop254><<<(unsigned)n, 32, Coop254::L::BYTES, st>>>(n, da1, da2, db1, db2, dok, ctx->d_flags);
+    else
+      k_bn254_pairing_check<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, da1, da2, db1, db2, dok, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
+  return rc == B2K_ERR_POINT ? B2K_OK : rc;   // a malformed operand already failed its own check
 }
 
 int b2k_bn254_g2_mul_batch(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return mul_batch_host<Bn254G2, false>(c, n, s, p, o); }

@@ -77,18 +77,16 @@ template <class CV, int NC, bool RANGE_CHECK, bool ORDER_CHECK>
 static int bn_unmarshal_check(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* ok) {
   if (!ctx || !in || !ok || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, pad256(n * (size_t)CV::IN_BYTES) + pad256(n) + 1024);
-  if (rc) return rc;
-  uint8_t* d_in = arena_take<uint8_t>(ctx, n * (size_t)CV::IN_BYTES);
-  uint8_t* d_ok = arena_take<uint8_t>(ctx, n);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemcpyAsync(d_in, in, n * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, st));
-  k_bn_unmarshal_check<CV, NC, RANGE_CHECK, ORDER_CHECK><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, d_in, d_ok);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return B2K_OK;
+  uint8_t *d_in = nullptr, *d_ok = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_in = c.in(in, n, CV::IN_BYTES);
+    d_ok = c.out(ok, n);
+  }, [&]() -> int {
+    k_bn_unmarshal_check<CV, NC, RANGE_CHECK, ORDER_CHECK><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(n, d_in, d_ok);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 extern "C" {

@@ -64,24 +64,16 @@ static int hash_host(b2k_ctx* ctx, int which, size_t n, const uint8_t* msgs, con
   if (!ctx || !msgs || !offsets || !out || n == 0) return B2K_ERR_ARG;
   if (which == 0 && (!dst || dst_len == 0 || dst_len > 255)) return B2K_ERR_ARG;
   if (which == 2 && (dst_len > 255 || (dst_len && !dst))) return B2K_ERR_ARG;
-  for (size_t i = 0; i < n; i++)
-    if (offsets[i + 1] < offsets[i]) { ctx->err = "message offsets must be non-decreasing"; return B2K_ERR_ARG; }
+  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  const size_t mbytes = offsets[n];
-  int rc = arena_reserve(ctx, mbytes + (n + 1) * 4 + 256 + n * 64 + 4096);
-  if (rc) return rc;
-  uint8_t* dm = arena_take<uint8_t>(ctx, mbytes + 1);
-  uint32_t* doff = arena_take<uint32_t>(ctx, n + 1);
-  uint8_t* dd = arena_take<uint8_t>(ctx, 256);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * 64);
-  if (mbytes) CK(cudaMemcpyAsync(dm, msgs, mbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(doff, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  if (which != 1 && dst_len) CK(cudaMemcpyAsync(dd, dst, dst_len, cudaMemcpyHostToDevice, ctx->stream));
-  rc = hash_dev(ctx, which, n, dm, doff, dd, dst_len, dout);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(out, dout, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return B2K_OK;
+  uint8_t *dm = nullptr, *dd = nullptr, *dout = nullptr;
+  uint32_t* doff = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    dm = c.in(msgs, offsets[n]);
+    doff = c.in(offsets, n + 1);
+    dd = c.in(dst, dst_len);
+    dout = c.out(out, n, 64);
+  }, [&] { return hash_dev(ctx, which, n, dm, doff, dd, dst_len, dout); });
 }
 
 extern "C" {

@@ -29,7 +29,6 @@ struct b2k_ctx {
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   b2k_arena arena;
-  b2k_arena arena_in;   // second arena: host-call inputs that must survive a nested call which re-reserves `arena` (bls.Verify wrappers)
   uint32_t* d_flags = nullptr;
   uint32_t* h_flags = nullptr;   // pinned
   cudaEvent_t ev[B2K_N_EV];
@@ -68,11 +67,10 @@ struct b2k_ctx {
 };
 
 // scratch arena (defined in b2k_api.cu): reserve resets the arena and grows it if needed;
-// take returns 256-byte aligned sub-buffers or nullptr.
+// take returns 256-byte aligned sub-buffers or nullptr.  A call reserves it at most once, through arena_carve, host_call or
+// msm_begin (host_call.cuh, msm_host.cuh), so nothing it has taken is handed out again while the call runs.
 int b2k_arena_reserve(b2k_ctx* ctx, size_t bytes);
 void* b2k_arena_take(b2k_ctx* ctx, size_t bytes);
-// the input arena: one buffer of at least `bytes` (grown on demand, never shrunk); nullptr on allocation failure
-void* b2k_arena_in(b2k_ctx* ctx, size_t bytes);
 
 // internal entry points shared between translation units (not part of include/b2kyber.h)
 extern "C" int b2k_internal_bls12381_g1_msm_buckets_host(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, void* b, size_t cap, int* plan);

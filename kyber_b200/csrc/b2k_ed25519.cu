@@ -35,19 +35,10 @@ int b2k_ed25519_mul_batch(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const 
   if (!ctx || !scalars || !points || !out || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   uint8_t *ds = nullptr, *dp = nullptr, *dout = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    ds = c.take<uint8_t>(n * 32);
-    dp = c.take<uint8_t>(n * 32);
-    dout = c.take<uint8_t>(n * 32);
-  });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  if ((rc = status_begin(ctx))) return rc;
-  CK(cudaMemcpyAsync(ds, scalars, n * 32, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dp, points, n * 32, cudaMemcpyHostToDevice, st));
-  rc = b2k_ed25519_mul_batch_dev(ctx, n, ds, dp, dout);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(out, dout, n * 32, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  return host_call(ctx, [&](Carve& c) {
+    ds = c.in(scalars, n, 32);
+    dp = c.in(points, n, 32);
+    dout = c.out(out, n, 32);
+  }, [&] { return b2k_ed25519_mul_batch_dev(ctx, n, ds, dp, dout); });
 }
 }  // extern "C"

@@ -286,71 +286,55 @@ int ed_recover_commit(b2k_ctx* ctx, size_t t, const uint32_t* indices, const uin
   ctx->launches += 1;
   if ((rc = ed_msm_enqueue(ctx, s, d_s, d_p, d_o))) return rc;
   CK(cudaMemcpyAsync(out, d_o, 32, cudaMemcpyDeviceToHost, st));
-  if ((rc = status_fetch_async(ctx))) return rc;
-  CK(cudaStreamSynchronize(st));
-  if (*ctx->h_flags & 4u) { ctx->err = "duplicate share index"; return B2K_ERR_ARG; }
-  return check_flags(ctx);
+  return status_finish(ctx);
 }
 
 int ed_pubpoly_eval(b2k_ctx* ctx, size_t t, const uint8_t* commits, size_t n, const uint32_t* indices, uint8_t* out) {
-  if (!ctx || !commits || !indices || !out || t == 0 || n == 0 || t >= (size_t(1) << 31) || n >= (size_t(1) << 31)) {
-    if (ctx) ctx->err = "bad argument";
-    return B2K_ERR_ARG;
-  }
+  if (!ctx || !commits || !indices || !out || t == 0 || n == 0 || t >= (size_t(1) << 31) || n >= (size_t(1) << 31))
+    return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   uint8_t *d_c = nullptr, *d_o = nullptr;
   EdNiels* d_cm = nullptr;
   uint32_t* d_idx = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_c = c.take<uint8_t>(t * 32);
+  return host_call(ctx, [&](Carve& c) {
+    d_c = c.in(commits, t, 32);
+    d_idx = c.in(indices, n);
     d_cm = c.take<EdNiels>(t);
-    d_idx = c.take<uint32_t>(n);
-    d_o = c.take<uint8_t>(n * 32);
+    d_o = c.out(out, n, 32);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_ed_load_niels<<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_c, d_cm, ctx->d_flags);
+    k_ed_pubpoly_eval<<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)t, d_cm, (uint32_t)n, d_idx, d_o);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return B2K_OK;
   });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  if ((rc = status_begin(ctx))) return rc;
-  CK(cudaMemcpyAsync(d_c, commits, t * 32, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_idx, indices, n * 4, cudaMemcpyHostToDevice, st));
-  k_ed_load_niels<<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_c, d_cm, ctx->d_flags);
-  k_ed_pubpoly_eval<<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)t, d_cm, (uint32_t)n, d_idx, d_o);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  CK(cudaMemcpyAsync(out, d_o, n * 32, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
 }
 
 int ed_pubpoly_check(b2k_ctx* ctx, size_t m, size_t t, const uint8_t* commits, size_t n, const uint32_t* indices,
                      const uint8_t* shares, uint8_t* ok) {
   if (!ctx || !commits || !indices || !shares || !ok || m == 0 || t == 0 || n == 0 || m * t >= (size_t(1) << 31) ||
-      m * n >= (size_t(1) << 31)) {
-    if (ctx) ctx->err = "bad argument";
-    return B2K_ERR_ARG;
-  }
+      m * n >= (size_t(1) << 31))
+    return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t mt = m * t, mn = m * n;
   uint8_t *d_c = nullptr, *d_s = nullptr, *d_ok = nullptr;
   EdNiels* d_cm = nullptr;
   uint32_t* d_idx = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_c = c.take<uint8_t>(mt * 32);
+  return host_call(ctx, [&](Carve& c) {
+    d_c = c.in(commits, mt, 32);
+    d_idx = c.in(indices, mn);
+    d_s = c.in(shares, mn, 32);
     d_cm = c.take<EdNiels>(mt);
-    d_idx = c.take<uint32_t>(mn);
-    d_s = c.take<uint8_t>(mn * 32);
-    d_ok = c.take<uint8_t>(mn);
+    d_ok = c.out(ok, mn);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_ed_load_niels<<<(unsigned)((mt + 255) / 256), 256, 0, st>>>(mt, d_c, d_cm, ctx->d_flags);
+    k_ed_pubpoly_check<<<(unsigned)((mn + 127) / 128), 128, 0, st>>>((uint32_t)m, (uint32_t)t, d_cm, (uint32_t)n, d_idx, d_s, d_ok);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return B2K_OK;
   });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  if ((rc = status_begin(ctx))) return rc;
-  CK(cudaMemcpyAsync(d_c, commits, mt * 32, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_idx, indices, mn * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_s, shares, mn * 32, cudaMemcpyHostToDevice, st));
-  k_ed_load_niels<<<(unsigned)((mt + 255) / 256), 256, 0, st>>>(mt, d_c, d_cm, ctx->d_flags);
-  k_ed_pubpoly_check<<<(unsigned)((mn + 127) / 128), 128, 0, st>>>((uint32_t)m, (uint32_t)t, d_cm, (uint32_t)n, d_idx, d_s, d_ok);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  CK(cudaMemcpyAsync(ok, d_ok, mn, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
 }
 
 }  // namespace

@@ -39,26 +39,15 @@ int b2k_ed25519_verify(b2k_ctx* ctx, size_t n, const uint8_t* pks, const uint8_t
   if (!ctx || !pks || !msgs || !offsets || !sigs || !status || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
-  const size_t mbytes = offsets[n];
-  const size_t o_pk = 0, o_sig = o_pk + n * 32, o_msg = o_sig + n * 64, o_off = (o_msg + mbytes + 15) & ~size_t(15),
-               o_st = o_off + (n + 1) * 4, total = o_st + n;
-  uint8_t* blob = (uint8_t*)b2k_arena_in(ctx, total);  // the context's input arena: one allocation, reused across calls
-  if (!blob) { ctx->err = "out of device memory"; return B2K_ERR_CUDA; }
-  cudaStream_t st = ctx->stream;
-  int rc = B2K_OK;
-  do {
-    if (cudaMemcpyAsync(blob + o_pk, pks, n * 32, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(blob + o_sig, sigs, n * 64, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        (mbytes && cudaMemcpyAsync(blob + o_msg, msgs, mbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
-        cudaMemcpyAsync(blob + o_off, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = B2K_ERR_CUDA; break; }
-    rc = b2k_ed25519_verify_dev(ctx, n, blob + o_pk, blob + o_msg, blob + o_off, blob + o_sig, blob + o_st);
-    if (rc) break;
-    if (cudaMemcpyAsync(status, blob + o_st, n, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) rc = B2K_ERR_CUDA;
-  } while (0);
-  cudaStreamSynchronize(st);
-  if (rc == B2K_ERR_CUDA) ctx->err = "CUDA failure in ed25519_verify";
-  return rc;
+  uint8_t *d_pk = nullptr, *d_sig = nullptr, *d_msg = nullptr, *d_st = nullptr;
+  uint32_t* d_off = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_pk = c.in(pks, n, 32);
+    d_sig = c.in(sigs, n, 64);
+    d_msg = c.in(msgs, offsets[n]);
+    d_off = c.in(offsets, n + 1);
+    d_st = c.out(status, n);
+  }, [&] { return b2k_ed25519_verify_dev(ctx, n, d_pk, d_msg, d_off, d_sig, d_st); });
 }
 
 }  // extern "C"

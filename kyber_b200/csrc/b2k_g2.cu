@@ -29,23 +29,17 @@ __global__ void __launch_bounds__(64) k_g2_decompress(size_t n, const uint8_t* _
 }
 }  // namespace b2k
 
-template <int IN, int OUT, class K>
-static int decompress_host(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok, K launch) {
+// stage the wire bytes, then the *_dev entry point
+template <class Dev>
+static int decompress_host(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok, size_t in_bytes, size_t out_bytes, Dev dev) {
   if (!ctx || !in || !out || !ok || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, n * (IN + OUT + 1) + 4096);
-  if (rc) return rc;
-  uint8_t* di = arena_take<uint8_t>(ctx, n * IN);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * OUT);
-  uint8_t* dk = arena_take<uint8_t>(ctx, n);
-  CK(cudaMemcpyAsync(di, in, n * IN, cudaMemcpyHostToDevice, ctx->stream));
-  launch(di, dout, dk);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, dout, n * OUT, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ok, dk, n, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return B2K_OK;
+  uint8_t *di = nullptr, *dout = nullptr, *dk = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    di = c.in(in, n, in_bytes);
+    dout = c.out(out, n, out_bytes);
+    dk = c.out(ok, n);
+  }, [&] { return dev(ctx, n, di, dout, dk); });
 }
 
 extern "C" {
@@ -66,14 +60,10 @@ int b2k_bls12381_g2_decompress_dev(b2k_ctx* ctx, size_t n, const void* in, void*
   return B2K_OK;
 }
 int b2k_bls12381_g1_decompress(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok) {
-  return decompress_host<48, 96>(ctx, n, in, out, ok, [&](uint8_t* di, uint8_t* dout, uint8_t* dk) {
-    k_g1_decompress<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(n, di, dout, dk, 1);
-  });
+  return decompress_host(ctx, n, in, out, ok, 48, 96, b2k_bls12381_g1_decompress_dev);
 }
 int b2k_bls12381_g2_decompress(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok) {
-  return decompress_host<96, 192>(ctx, n, in, out, ok, [&](uint8_t* di, uint8_t* dout, uint8_t* dk) {
-    k_g2_decompress<<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(n, di, dout, dk, 1);
-  });
+  return decompress_host(ctx, n, in, out, ok, 96, 192, b2k_bls12381_g2_decompress_dev);
 }
 int b2k_bls12381_g2_mul_batch(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return mul_batch_host<Bls381G2, false>(c, n, s, p, o); }
 int b2k_bls12381_g2_mul_batch_affine(b2k_ctx* c, size_t n, const uint8_t* s, const uint8_t* p, uint8_t* o) { return mul_batch_host<Bls381G2, true>(c, n, s, p, o); }

@@ -318,109 +318,89 @@ void launch_gt_exp(const b2k_ctx* ctx, size_t n, const uint8_t* ds, const uint8_
 
 template <class P>
 int gt_binary(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* a, const uint8_t* b, uint8_t* out, int op) {
-  if (!ctx || !a || !out || n == 0 || (op == 0 && !b) || (op == 2 && !scalars)) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !a || !out || n == 0 || (op == 0 && !b) || (op == 2 && !scalars)) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   const size_t gb = (size_t)P::GT_BYTES;
-  int rc = arena_reserve(ctx, 3 * pad256(n * gb) + pad256(n * 32) + 1024);
-  if (rc) return rc;
-  uint8_t* da = arena_take<uint8_t>(ctx, n * gb);
-  uint8_t* db = arena_take<uint8_t>(ctx, n * gb);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * gb);
-  uint8_t* ds = arena_take<uint8_t>(ctx, n * 32);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(da, a, n * gb, cudaMemcpyHostToDevice, st));
-  const unsigned grid = (unsigned)((n + 63) / 64);
-  if (op == 0) {
-    CK(cudaMemcpyAsync(db, b, n * gb, cudaMemcpyHostToDevice, st));
-    k_gt_mul<P><<<grid, 64, 0, st>>>(n, da, db, dout, ctx->d_flags);
-  } else if (op == 1) {
-    k_gt_inv<P><<<grid, 64, 0, st>>>(n, da, dout, ctx->d_flags);
-  } else {
-    CK(cudaMemcpyAsync(ds, scalars, n * 32, cudaMemcpyHostToDevice, st));
-    launch_gt_exp<P>(ctx, n, ds, da, dout);
-  }
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, dout, n * gb, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *da = nullptr, *db = nullptr, *ds = nullptr, *dout = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    da = c.in(a, n, gb);
+    db = c.in(b, op == 0 ? n : 0, gb);
+    ds = c.in(scalars, op == 2 ? n : 0, 32);
+    dout = c.out(out, n, gb);
+  }, [&]() -> int {
+    const unsigned grid = (unsigned)((n + 63) / 64);
+    if (op == 0) k_gt_mul<P><<<grid, 64, 0, ctx->stream>>>(n, da, db, dout, ctx->d_flags);
+    else if (op == 1) k_gt_inv<P><<<grid, 64, 0, ctx->stream>>>(n, da, dout, ctx->d_flags);
+    else launch_gt_exp<P>(ctx, n, ds, da, dout);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 template <class P>
 int miller_host(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* out) {
-  if (!ctx || !g1 || !g2 || !out || n == 0) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !g1 || !g2 || !out || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t b1 = (size_t)P::G1::IN_BYTES, b2 = (size_t)P::G2::IN_BYTES, gb = (size_t)P::GT_BYTES;
-  int rc = arena_reserve(ctx, pad256(n * b1) + pad256(n * b2) + pad256(n * gb) + 1024);
-  if (rc) return rc;
-  uint8_t* d1 = arena_take<uint8_t>(ctx, n * b1);
-  uint8_t* d2 = arena_take<uint8_t>(ctx, n * b2);
-  uint8_t* dg = arena_take<uint8_t>(ctx, n * gb);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d1, g1, n * b1, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d2, g2, n * b2, cudaMemcpyHostToDevice, st));
-  k_miller<P><<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, d1, d2, dg, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, dg, n * gb, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d1 = nullptr, *d2 = nullptr, *dg = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d1 = c.in(g1, n, P::G1::IN_BYTES);
+    d2 = c.in(g2, n, P::G2::IN_BYTES);
+    dg = c.out(out, n, P::GT_BYTES);
+  }, [&]() -> int {
+    k_miller<P><<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(n, d1, d2, dg, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 template <class P>
 int final_exp_host(b2k_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out) {
-  if (!ctx || !in || !out || n == 0) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !in || !out || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t gb = (size_t)P::GT_BYTES;
-  int rc = arena_reserve(ctx, 2 * pad256(n * gb) + 1024);
-  if (rc) return rc;
-  uint8_t* di = arena_take<uint8_t>(ctx, n * gb);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * gb);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(di, in, n * gb, cudaMemcpyHostToDevice, st));
-  k_final_exp<P><<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, di, dout, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, dout, n * gb, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *di = nullptr, *dout = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    di = c.in(in, n, P::GT_BYTES);
+    dout = c.out(out, n, P::GT_BYTES);
+  }, [&]() -> int {
+    k_final_exp<P><<<(unsigned)((n + 63) / 64), 64, 0, ctx->stream>>>(n, di, dout, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 // ok[0] = (prod_i e(g1_i, g2_i) == 1); gt (optional) = the product's bytes
 template <class P>
 int product_check_host(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* ok, uint8_t* gt) {
   using F12 = typename P::F12;
-  if (!ctx || !g1 || !g2 || (!ok && !gt) || n == 0 || n >= (size_t(1) << 31)) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !g1 || !g2 || (!ok && !gt) || n == 0 || n >= (size_t(1) << 31)) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t b1 = (size_t)P::G1::IN_BYTES, b2 = (size_t)P::G2::IN_BYTES, gb = (size_t)P::GT_BYTES;
+  const size_t gb = (size_t)P::GT_BYTES;
   size_t nblk = (n + b2k::PROD_BLOCK - 1) / b2k::PROD_BLOCK;
   if (nblk > 4096) nblk = 4096;                                              // beyond that a thread multiplies several values
-  int rc = arena_reserve(ctx, pad256(n * b1) + pad256(n * b2) + pad256(n * gb) + pad256(nblk * sizeof(F12)) + 2 * pad256(gb) + 2048);
-  if (rc) return rc;
-  uint8_t* d1 = arena_take<uint8_t>(ctx, n * b1);
-  uint8_t* d2 = arena_take<uint8_t>(ctx, n * b2);
-  uint8_t* dm = arena_take<uint8_t>(ctx, n * gb);
-  F12* parts = arena_take<F12>(ctx, nblk);
-  uint8_t* df = arena_take<uint8_t>(ctx, gb);
-  uint8_t* dgt = arena_take<uint8_t>(ctx, gb);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d1, g1, n * b1, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d2, g2, n * b2, cudaMemcpyHostToDevice, st));
-  const size_t smem = b2k::PROD_BLOCK * sizeof(F12);
-  k_miller<P><<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, d1, d2, dm, ctx->d_flags);
-  k_gt_block_product<P><<<(unsigned)nblk, b2k::PROD_BLOCK, smem, st>>>(n, dm, parts);
-  k_product_tree<P><<<1, b2k::PROD_BLOCK, smem, st>>>(nblk, parts, df);
-  k_final_exp<P><<<1, 64, 0, st>>>(1, df, dgt, ctx->d_flags);               // ONE final exponentiation
-  CK(cudaGetLastError());
-  ctx->launches += 4;
   uint8_t hgt[576];
-  CK(cudaMemcpyAsync(gt ? gt : hgt, dgt, gb, cudaMemcpyDeviceToHost, st));
-  rc = status_finish(ctx);
+  uint8_t *d1 = nullptr, *d2 = nullptr, *dm = nullptr, *df = nullptr, *dgt = nullptr;
+  F12* parts = nullptr;
+  const int rc = host_call(ctx, [&](Carve& c) {
+    d1 = c.in(g1, n, P::G1::IN_BYTES);
+    d2 = c.in(g2, n, P::G2::IN_BYTES);
+    dm = c.take<uint8_t>(n, gb);
+    parts = c.take<F12>(nblk);
+    df = c.take<uint8_t>(gb);
+    dgt = c.out(gt ? gt : hgt, gb);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    const size_t smem = b2k::PROD_BLOCK * sizeof(F12);
+    k_miller<P><<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, d1, d2, dm, ctx->d_flags);
+    k_gt_block_product<P><<<(unsigned)nblk, b2k::PROD_BLOCK, smem, st>>>(n, dm, parts);
+    k_product_tree<P><<<1, b2k::PROD_BLOCK, smem, st>>>(nblk, parts, df);
+    k_final_exp<P><<<1, 64, 0, st>>>(1, df, dgt, ctx->d_flags);               // ONE final exponentiation
+    CK(cudaGetLastError());
+    ctx->launches += 4;
+    return B2K_OK;
+  });
   if (rc) return rc;
   if (ok) {
     const uint8_t* e = gt ? gt : hgt;                                      // GT one = 0 ... 0 1 (only the last coefficient, c0.c0.c0)
@@ -433,24 +413,19 @@ int product_check_host(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t*
 
 template <class CV>
 int add_batch_host(b2k_ctx* ctx, size_t n, const uint8_t* a, const uint8_t* b, int negate_b, uint8_t* out) {
-  if (!ctx || !a || !b || !out || n == 0) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !a || !b || !out || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t pb = (size_t)CV::IN_BYTES;
-  int rc = arena_reserve(ctx, 3 * pad256(n * pb) + 1024);
-  if (rc) return rc;
-  uint8_t* da = arena_take<uint8_t>(ctx, n * pb);
-  uint8_t* db = arena_take<uint8_t>(ctx, n * pb);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * pb);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(da, a, n * pb, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(db, b, n * pb, cudaMemcpyHostToDevice, st));
-  k_add_batch<CV><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, da, db, negate_b, dout, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, dout, n * pb, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *da = nullptr, *db = nullptr, *dout = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    da = c.in(a, n, CV::IN_BYTES);
+    db = c.in(b, n, CV::IN_BYTES);
+    dout = c.out(out, n, CV::IN_BYTES);
+  }, [&]() -> int {
+    k_add_batch<CV><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(n, da, db, negate_b, dout, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 }  // namespace

@@ -49,7 +49,8 @@ __global__ void k_and_flags(size_t n, const uint8_t* a, const uint8_t* b, uint8_
   if (i < n) out[i] = a[i] & b[i];
 }
 
-// same kernels as b2k_g2.cu, local to this translation unit
+// the decompression kernels of b2k_g2.cu, built here without B2K_FP2_BYREF: that build of the G2 kernel takes a 2608-byte stack
+// frame against 2112 bytes here, and a one-signature verify_g1sig through it measured ~1 % slower (H100 80GB HBM3, 700 W)
 __global__ void __launch_bounds__(128) k_g1_decompress_v(size_t n, const uint8_t* __restrict__ in, uint8_t* __restrict__ out,
                                                          uint8_t* __restrict__ ok) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -73,6 +74,105 @@ __global__ void __launch_bounds__(64) k_g2_decompress_v(size_t n, const uint8_t*
 
 }  // namespace b2k
 
+namespace {
+
+// hash_to_g1/g2 from host buffers: out_bytes per point, dev = the *_dev entry point
+template <class Dev>
+int hash_host(b2k_ctx* ctx, size_t n, const uint8_t* msgs, const uint32_t* offsets, const uint8_t* dst, uint32_t dst_len, uint8_t* out,
+              size_t out_bytes, Dev dev) {
+  if (!ctx || !msgs || !offsets || !dst || !out || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
+  uint8_t *dm = nullptr, *dd = nullptr, *dout = nullptr;
+  uint32_t* doff = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    dm = c.in(msgs, offsets[n]);
+    doff = c.in(offsets, n + 1);
+    dd = c.in(dst, dst_len);
+    dout = c.out(out, n, out_bytes);
+  }, [&] { return dev(ctx, n, dm, doff, dd, dst_len, dout); });
+}
+
+// scratch of bls.Verify for n signatures: decompressed keys and signatures, H(m) (in the signature's group), the decode flags
+// and the generator (in the key's group)
+struct VerifyScratch {
+  uint8_t *pk, *sg, *hm, *ok1, *ok2, *okc, *gen;
+};
+void verify_layout(Carve& c, VerifyScratch& s, size_t n, bool sig_g1) {
+  const size_t pk_bytes = sig_g1 ? 192 : 96, sig_bytes = sig_g1 ? 96 : 192;
+  s.pk = c.take<uint8_t>(n, pk_bytes);
+  s.sg = c.take<uint8_t>(n, sig_bytes);
+  s.hm = c.take<uint8_t>(n, sig_bytes);
+  s.ok1 = c.take<uint8_t>(n);
+  s.ok2 = c.take<uint8_t>(n);
+  s.okc = c.take<uint8_t>(n);
+  s.gen = c.take<uint8_t>(pk_bytes);
+}
+
+// ok[i] = bls.Verify(pk_i, msg_i, sig_i), every buffer on the device:
+//   sig_g1: UnmarshalBinary(pk in G2), UnmarshalBinary(sig in G1), H(msg) in G1, e(H(m), pk) == e(sig, G2 generator)
+//   else (bls.NewSchemeOnG2, sign/bls/bls.go:48-59): pk in G1, sig in G2, H(msg) in G2, e(pk, H(m)) == e(G1 base, sig)
+int verify_enqueue(b2k_ctx* ctx, bool sig_g1, const VerifyScratch& s, size_t n, const void* pks, const void* msgs, const void* offsets,
+                   const void* dst, uint32_t dst_len, const void* sigs, void* ok) {
+  cudaStream_t st = ctx->stream;
+  const uint8_t *m = (const uint8_t*)msgs, *d = (const uint8_t*)dst;
+  const uint32_t* o = (const uint32_t*)offsets;
+  const uint8_t *p = (const uint8_t*)pks, *g = (const uint8_t*)sigs;
+  if (sig_g1) {
+    k_write_g2_generator<<<1, 32, 0, st>>>(s.gen);
+    k_g2_decompress_v<<<blocks_of(n, 64), 64, 0, st>>>(n, p, s.pk, s.ok1);
+    k_g1_decompress_v<<<blocks_of(n, 128), 128, 0, st>>>(n, g, s.sg, s.ok2);
+  } else {
+    k_write_g1_generator<<<1, 32, 0, st>>>(s.gen);
+    k_g1_decompress_v<<<blocks_of(n, 128), 128, 0, st>>>(n, p, s.pk, s.ok1);
+    k_g2_decompress_v<<<blocks_of(n, 64), 64, 0, st>>>(n, g, s.sg, s.ok2);
+  }
+  k_and_flags<<<blocks_of(n, 256), 256, 0, st>>>(n, s.ok1, s.ok2, s.okc);
+  if (sig_g1) {
+    k_hash_to_g1<<<blocks_of(n, 128), 128, 0, st>>>(n, m, o, d, dst_len, s.hm);
+    b2k_internal_launch_pairing_check(ctx, n, s.hm, s.pk, s.sg, s.gen, (uint8_t*)ok, 1, s.okc);
+  } else {
+    k_hash_to_g2<<<blocks_of(n, 64), 64, 0, st>>>(n, m, o, d, dst_len, s.hm);
+    b2k_internal_launch_pairing_check(ctx, n, s.pk, s.hm, s.gen, s.sg, (uint8_t*)ok, 2, s.okc);   // b = (base [shared], sig)
+  }
+  CK(cudaGetLastError());
+  ctx->launches += 6;
+  return B2K_OK;
+}
+
+int verify_dev(b2k_ctx* ctx, bool sig_g1, size_t n, const void* d_pks, const void* d_msgs, const void* d_offsets, const void* d_dst,
+               uint32_t dst_len, const void* d_sigs, void* d_ok) {
+  if (!ctx || !d_pks || !d_msgs || !d_offsets || !d_dst || !d_sigs || !d_ok || n == 0 || dst_len == 0 || dst_len > 255)
+    return B2K_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  VerifyScratch s;
+  int rc = arena_carve(ctx, [&](Carve& c) { verify_layout(c, s, n, sig_g1); });
+  if (rc) return rc;
+  return verify_enqueue(ctx, sig_g1, s, n, d_pks, d_msgs, d_offsets, d_dst, dst_len, d_sigs, d_ok);
+}
+
+int verify_host(b2k_ctx* ctx, bool sig_g1, size_t n, const uint8_t* pks, const uint8_t* msgs, const uint32_t* offsets, const uint8_t* dst,
+                uint32_t dst_len, const uint8_t* sigs, uint8_t* ok) {
+  if (!ctx || !pks || !msgs || !offsets || !dst || !sigs || !ok || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
+  VerifyScratch s;
+  uint8_t *d_pk = nullptr, *d_sig = nullptr, *d_msg = nullptr, *d_dst = nullptr, *d_ok = nullptr;
+  uint32_t* d_off = nullptr;
+  const int rc = host_call(ctx, [&](Carve& c) {
+    d_pk = c.in(pks, n, sig_g1 ? 96 : 48);
+    d_sig = c.in(sigs, n, sig_g1 ? 48 : 96);
+    d_msg = c.in(msgs, offsets[n]);
+    d_off = c.in(offsets, n + 1);
+    d_dst = c.in(dst, dst_len);
+    d_ok = c.out(ok, n);
+    verify_layout(c, s, n, sig_g1);
+  }, [&] { return verify_enqueue(ctx, sig_g1, s, n, d_pk, d_msg, d_off, d_dst, dst_len, d_sig, d_ok); });
+  return rc == B2K_ERR_POINT ? B2K_OK : rc;   // a malformed operand already failed its own check: per-element booleans
+}
+
+}  // namespace
+
 extern "C" {
 
 int b2k_bls12381_hash_to_g1_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, const void* d_offsets, const void* d_dst,
@@ -88,54 +188,7 @@ int b2k_bls12381_hash_to_g1_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, cons
 
 int b2k_bls12381_hash_to_g1(b2k_ctx* ctx, size_t n, const uint8_t* msgs, const uint32_t* offsets, const uint8_t* dst,
                             uint32_t dst_len, uint8_t* out) {
-  if (!ctx || !msgs || !offsets || !dst || !out || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
-  size_t mbytes = offsets[n];
-  int rc = arena_reserve(ctx, mbytes + (n + 1) * 4 + 256 + n * 96 + 4096);
-  if (rc) return rc;
-  uint8_t* dm = arena_take<uint8_t>(ctx, mbytes + 1);
-  uint32_t* doff = arena_take<uint32_t>(ctx, n + 1);
-  uint8_t* dd = arena_take<uint8_t>(ctx, 256);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * 96);
-  if (mbytes) CK(cudaMemcpyAsync(dm, msgs, mbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(doff, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(dd, dst, dst_len, cudaMemcpyHostToDevice, ctx->stream));
-  rc = b2k_bls12381_hash_to_g1_dev(ctx, n, dm, doff, dd, dst_len, dout);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(out, dout, n * 96, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return B2K_OK;
-}
-
-// ok[i] = bls.Verify(pk_i, msg_i, sig_i) for signatures on G1 / keys on G2:
-//   UnmarshalBinary(pk) , UnmarshalBinary(sig) , H(msg) , e(H(m), pk) == e(sig, G2 generator)
-// All buffers are DEVICE pointers; scratch comes from the context arena.
-int b2k_bls12381_verify_g1sig_dev(b2k_ctx* ctx, size_t n, const void* d_pks96, const void* d_msgs, const void* d_offsets,
-                                  const void* d_dst, uint32_t dst_len, const void* d_sigs48, void* d_ok) {
-  if (!ctx || !d_pks96 || !d_msgs || !d_offsets || !d_dst || !d_sigs48 || !d_ok || n == 0 || dst_len == 0 || dst_len > 255)
-    return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, n * (192 + 96 + 96 + 3) + 8192);
-  if (rc) return rc;
-  uint8_t* pk = arena_take<uint8_t>(ctx, n * 192);
-  uint8_t* sg = arena_take<uint8_t>(ctx, n * 96);
-  uint8_t* hm = arena_take<uint8_t>(ctx, n * 96);
-  uint8_t* ok1 = arena_take<uint8_t>(ctx, n);
-  uint8_t* ok2 = arena_take<uint8_t>(ctx, n);
-  uint8_t* okc = arena_take<uint8_t>(ctx, n);
-  uint8_t* gen = arena_take<uint8_t>(ctx, 192);
-  cudaStream_t st = ctx->stream;
-  k_write_g2_generator<<<1, 32, 0, st>>>(gen);
-  k_g2_decompress_v<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, (const uint8_t*)d_pks96, pk, ok1);
-  k_g1_decompress_v<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, (const uint8_t*)d_sigs48, sg, ok2);
-  k_and_flags<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, ok1, ok2, okc);
-  k_hash_to_g1<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, (const uint8_t*)d_msgs, (const uint32_t*)d_offsets,
-                                                          (const uint8_t*)d_dst, dst_len, hm);
-  b2k_internal_launch_pairing_check(ctx, n, hm, pk, sg, gen, (uint8_t*)d_ok, 1, okc);
-  CK(cudaGetLastError());
-  ctx->launches += 6;
-  return B2K_OK;
+  return hash_host(ctx, n, msgs, offsets, dst, dst_len, out, 96, b2k_bls12381_hash_to_g1_dev);
 }
 
 int b2k_bls12381_hash_to_g2_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, const void* d_offsets, const void* d_dst,
@@ -151,115 +204,26 @@ int b2k_bls12381_hash_to_g2_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, cons
 
 int b2k_bls12381_hash_to_g2(b2k_ctx* ctx, size_t n, const uint8_t* msgs, const uint32_t* offsets, const uint8_t* dst,
                             uint32_t dst_len, uint8_t* out) {
-  if (!ctx || !msgs || !offsets || !dst || !out || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
-  size_t mbytes = offsets[n];
-  int rc = arena_reserve(ctx, mbytes + (n + 1) * 4 + 256 + n * 192 + 4096);
-  if (rc) return rc;
-  uint8_t* dm = arena_take<uint8_t>(ctx, mbytes + 1);
-  uint32_t* doff = arena_take<uint32_t>(ctx, n + 1);
-  uint8_t* dd = arena_take<uint8_t>(ctx, 256);
-  uint8_t* dout = arena_take<uint8_t>(ctx, n * 192);
-  if (mbytes) CK(cudaMemcpyAsync(dm, msgs, mbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(doff, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(dd, dst, dst_len, cudaMemcpyHostToDevice, ctx->stream));
-  rc = b2k_bls12381_hash_to_g2_dev(ctx, n, dm, doff, dd, dst_len, dout);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(out, dout, n * 192, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return B2K_OK;
+  return hash_host(ctx, n, msgs, offsets, dst, dst_len, out, 192, b2k_bls12381_hash_to_g2_dev);
 }
 
-// ok[i] = bls.Verify for the scheme with signatures on G2 / keys on G1 (bls.NewSchemeOnG2, sign/bls/bls.go:48-59):
-//   UnmarshalBinary(pk in G1), UnmarshalBinary(sig in G2), H(msg) in G2, e(G1 base, sig) == e(pk, H(m))
+// bls.Verify, sign/bls/bls.go:82-96, for signatures on G1 / keys on G2 (g1sig) and signatures on G2 / keys on G1 (g2sig).
+// The *_dev forms take device buffers; scratch comes from the context arena.
+int b2k_bls12381_verify_g1sig_dev(b2k_ctx* ctx, size_t n, const void* d_pks96, const void* d_msgs, const void* d_offsets,
+                                  const void* d_dst, uint32_t dst_len, const void* d_sigs48, void* d_ok) {
+  return verify_dev(ctx, true, n, d_pks96, d_msgs, d_offsets, d_dst, dst_len, d_sigs48, d_ok);
+}
 int b2k_bls12381_verify_g2sig_dev(b2k_ctx* ctx, size_t n, const void* d_pks48, const void* d_msgs, const void* d_offsets,
                                   const void* d_dst, uint32_t dst_len, const void* d_sigs96, void* d_ok) {
-  if (!ctx || !d_pks48 || !d_msgs || !d_offsets || !d_dst || !d_sigs96 || !d_ok || n == 0 || dst_len == 0 || dst_len > 255)
-    return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, n * (96 + 192 + 192 + 3) + 8192);
-  if (rc) return rc;
-  uint8_t* pk = arena_take<uint8_t>(ctx, n * 96);
-  uint8_t* sg = arena_take<uint8_t>(ctx, n * 192);
-  uint8_t* hm = arena_take<uint8_t>(ctx, n * 192);
-  uint8_t* ok1 = arena_take<uint8_t>(ctx, n);
-  uint8_t* ok2 = arena_take<uint8_t>(ctx, n);
-  uint8_t* okc = arena_take<uint8_t>(ctx, n);
-  uint8_t* gen = arena_take<uint8_t>(ctx, 96);
-  cudaStream_t st = ctx->stream;
-  k_write_g1_generator<<<1, 32, 0, st>>>(gen);
-  k_g1_decompress_v<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, (const uint8_t*)d_pks48, pk, ok1);
-  k_g2_decompress_v<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, (const uint8_t*)d_sigs96, sg, ok2);
-  k_and_flags<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, ok1, ok2, okc);
-  k_hash_to_g2<<<(unsigned)((n + 63) / 64), 64, 0, st>>>(n, (const uint8_t*)d_msgs, (const uint32_t*)d_offsets,
-                                                        (const uint8_t*)d_dst, dst_len, hm);
-  // e(pk, H(m)) == e(base, sig): a = (pk, hm), b = (base [shared], sig)
-  b2k_internal_launch_pairing_check(ctx, n, pk, hm, gen, sg, (uint8_t*)d_ok, 2, okc);
-  CK(cudaGetLastError());
-  ctx->launches += 6;
-  return B2K_OK;
+  return verify_dev(ctx, false, n, d_pks48, d_msgs, d_offsets, d_dst, dst_len, d_sigs96, d_ok);
 }
-
-int b2k_bls12381_verify_g2sig(b2k_ctx* ctx, size_t n, const uint8_t* pks48, const uint8_t* msgs, const uint32_t* offsets,
-                              const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs96, uint8_t* ok) {
-  if (!ctx || !pks48 || !msgs || !offsets || !dst || !sigs96 || !ok || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  size_t mbytes = offsets[n];
-  uint8_t* blob = nullptr;
-  size_t o_pk = 0, o_sig = o_pk + n * 48, o_msg = o_sig + n * 96, o_off = (o_msg + mbytes + 15) & ~size_t(15),
-         o_dst = o_off + (n + 1) * 4, o_ok = o_dst + 256, total = o_ok + n;
-  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
-  blob = (uint8_t*)b2k_arena_in(ctx, total);        // the context's input arena (no cudaMalloc / cudaFree per call: both synchronise the device)
-  if (!blob) { ctx->err = "out of device memory"; return B2K_ERR_CUDA; }
-  cudaStream_t st = ctx->stream;
-  int rc = B2K_OK;
-  do {
-    if (cudaMemcpyAsync(blob + o_pk, pks48, n * 48, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(blob + o_sig, sigs96, n * 96, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        (mbytes && cudaMemcpyAsync(blob + o_msg, msgs, mbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
-        cudaMemcpyAsync(blob + o_off, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(blob + o_dst, dst, dst_len, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = B2K_ERR_CUDA; break; }
-    rc = b2k_bls12381_verify_g2sig_dev(ctx, n, blob + o_pk, blob + o_msg, blob + o_off, blob + o_dst, dst_len,
-                                       blob + o_sig, blob + o_ok);
-    if (rc) break;
-    if (cudaMemcpyAsync(ok, blob + o_ok, n, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) rc = B2K_ERR_CUDA;
-  } while (0);
-  cudaStreamSynchronize(st);
-  if (rc == B2K_ERR_CUDA) ctx->err = "CUDA failure in verify_g2sig";
-  return rc;
-}
-
 int b2k_bls12381_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* pks96, const uint8_t* msgs, const uint32_t* offsets,
                               const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs48, uint8_t* ok) {
-  if (!ctx || !pks96 || !msgs || !offsets || !dst || !sigs48 || !ok || n == 0 || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  size_t mbytes = offsets[n];
-  // inputs live in a separate allocation because verify_dev re-reserves the arena
-  uint8_t* blob = nullptr;
-  size_t o_pk = 0, o_sig = o_pk + n * 96, o_msg = o_sig + n * 48, o_off = (o_msg + mbytes + 15) & ~size_t(15),
-         o_dst = o_off + (n + 1) * 4, o_ok = o_dst + 256, total = o_ok + n;
-  if (check_offsets(ctx, n, offsets)) return B2K_ERR_ARG;
-  blob = (uint8_t*)b2k_arena_in(ctx, total);        // the context's input arena (no cudaMalloc / cudaFree per call: both synchronise the device)
-  if (!blob) { ctx->err = "out of device memory"; return B2K_ERR_CUDA; }
-  cudaStream_t st = ctx->stream;
-  int rc = B2K_OK;
-  do {
-    if (cudaMemcpyAsync(blob + o_pk, pks96, n * 96, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(blob + o_sig, sigs48, n * 48, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        (mbytes && cudaMemcpyAsync(blob + o_msg, msgs, mbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
-        cudaMemcpyAsync(blob + o_off, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(blob + o_dst, dst, dst_len, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = B2K_ERR_CUDA; break; }
-    rc = b2k_bls12381_verify_g1sig_dev(ctx, n, blob + o_pk, blob + o_msg, blob + o_off, blob + o_dst, dst_len,
-                                       blob + o_sig, blob + o_ok);
-    if (rc) break;
-    if (cudaMemcpyAsync(ok, blob + o_ok, n, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) rc = B2K_ERR_CUDA;
-  } while (0);
-  cudaStreamSynchronize(st);
-  if (rc == B2K_ERR_CUDA) ctx->err = "CUDA failure in verify_g1sig";
-  return rc;
+  return verify_host(ctx, true, n, pks96, msgs, offsets, dst, dst_len, sigs48, ok);
+}
+int b2k_bls12381_verify_g2sig(b2k_ctx* ctx, size_t n, const uint8_t* pks48, const uint8_t* msgs, const uint32_t* offsets,
+                              const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs96, uint8_t* ok) {
+  return verify_host(ctx, false, n, pks48, msgs, offsets, dst, dst_len, sigs96, ok);
 }
 
 }  // extern "C"

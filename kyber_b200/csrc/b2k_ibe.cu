@@ -17,8 +17,6 @@ extern "C" void b2k_internal_launch_bls12381_gt_exp(const b2k_ctx* c, size_t n, 
 
 namespace b2k {
 
-constexpr uint32_t FLAG_IBE_H3 = 64u;          // H3 found no scalar below r (rejection sampling failure)
-
 template <class CV> struct IbeCodec;
 template <> struct IbeCodec<Bls381G1> {
   B2K_D static bool decompress(Affine<BFp>& a, const uint8_t* in) { return g1_decompress(a, in, true); }
@@ -127,78 +125,66 @@ namespace {
 constexpr uint8_t DST_G1[] = "BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_NUL_";
 constexpr uint8_t DST_G2[] = "BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_NUL_";
 
-unsigned blocks(size_t n, unsigned b) { return (unsigned)((n + b - 1) / b); }
-
 // gt[i] = e(g1[i], q) for one G2 point q (operand form) through the line table
-int pair_fixed_q(b2k_ctx* ctx, size_t n, const uint8_t* d_g1, const uint8_t* d_q, uint8_t* d_gt) {
-  BlsLineCoef* tab = arena_take<BlsLineCoef>(ctx, BLS_MILLER_STEPS);
-  uint32_t* live = arena_take<uint32_t>(ctx, 1);
-  if (!live) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
+void fixed_q_layout(Carve& c, BlsLineCoef*& tab, uint32_t*& live) {
+  tab = c.take<BlsLineCoef>(BLS_MILLER_STEPS);
+  live = c.take<uint32_t>(1);
+}
+int pair_fixed_q(b2k_ctx* ctx, size_t n, const uint8_t* d_g1, const uint8_t* d_q, BlsLineCoef* tab, uint32_t* live, uint8_t* d_gt) {
   k_ibe_line_table<<<1, 32, 0, ctx->stream>>>(d_q, tab, live, ctx->d_flags);
-  k_ibe_pair_fixed_q<<<blocks(n, 64), 64, 0, ctx->stream>>>(n, d_g1, tab, live, d_gt, ctx->d_flags);
+  k_ibe_pair_fixed_q<<<blocks_of(n, 64), 64, 0, ctx->stream>>>(n, d_g1, tab, live, d_gt, ctx->d_flags);
   CK(cudaGetLastError());
   ctx->launches += 2;
   return B2K_OK;
 }
-constexpr size_t FIXED_Q_SCRATCH = 2 * 256 + BLS_MILLER_STEPS * sizeof(BlsLineCoef);
 
 // DecryptCCAonG1 (KEY = G2, U on G1) / DecryptCCAonG2 (KEY = G1, U on G2)
 template <class UG, class KG>
 int ibe_decrypt(b2k_ctx* ctx, const uint8_t* priv, size_t n, const uint8_t* u, size_t len, const uint8_t* v, const uint8_t* w, uint8_t* msg,
                 uint8_t* status) {
   if (!ctx) return B2K_ERR_ARG;
-  if (!priv || !u || !status || n == 0 || n >= (size_t(1) << 31) || len > IBE_MAX_LEN || (len && (!v || !w || !msg))) {
-    ctx->err = "bad argument (n >= 1, len <= 32)";
-    return B2K_ERR_ARG;
-  }
+  if (!priv || !u || !status || n == 0 || n >= (size_t(1) << 31) || len > IBE_MAX_LEN || (len && (!v || !w || !msg)))
+    return bad_arg(ctx, "bad argument (n >= 1, len <= 32)");
   CK(cudaSetDevice(ctx->device));
   constexpr bool u_on_g1 = UG::OUT_BYTES == 48;
   const bool fixed_q = u_on_g1 && !(ctx->coop_max_n > 0 && n <= (size_t)ctx->coop_max_n);
-  const size_t lb = len ? len : 1;
-  int rc = arena_reserve(ctx, pad256(KG::OUT_BYTES) + pad256(n * UG::OUT_BYTES) + pad256(n * UG::IN_BYTES) + 2 * pad256(n) +
-                                  3 * pad256(n * lb) + pad256((fixed_q ? 1 : n) * KG::IN_BYTES) + pad256(n * 576) + FIXED_Q_SCRATCH + 4096);
-  if (rc) return rc;
-  uint8_t* d_key = arena_take<uint8_t>(ctx, KG::OUT_BYTES);
-  uint8_t* d_uw = arena_take<uint8_t>(ctx, n * UG::OUT_BYTES);
-  uint8_t* d_u = arena_take<uint8_t>(ctx, n * UG::IN_BYTES);
-  uint8_t* d_ok = arena_take<uint8_t>(ctx, n);
-  uint8_t* d_st = arena_take<uint8_t>(ctx, n);
-  uint8_t* d_v = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_w = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_m = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_keys = arena_take<uint8_t>(ctx, (fixed_q ? 1 : n) * KG::IN_BYTES);
-  uint8_t* d_gt = arena_take<uint8_t>(ctx, n * 576);
-  if (!d_gt) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d_key, priv, KG::OUT_BYTES, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_uw, u, n * UG::OUT_BYTES, cudaMemcpyHostToDevice, st));
-  if (len) {
-    CK(cudaMemcpyAsync(d_v, v, n * len, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_w, w, n * len, cudaMemcpyHostToDevice, st));
-  }
   const size_t copies = fixed_q ? 1 : n;
-  const unsigned kb = blocks(copies * KG::IN_BYTES, 256);
-  k_ibe_key<KG><<<kb < 1024 ? kb : 1024, 256, 0, st>>>(d_key, copies, d_keys, ctx->d_flags);
-  k_ibe_decode<UG><<<blocks(n, 64), 64, 0, st>>>(n, d_uw, d_u, d_ok);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  if (fixed_q) {
-    rc = pair_fixed_q(ctx, n, d_u, d_keys, d_gt);
-    if (rc) return rc;
-  } else {
-    if (u_on_g1) b2k_internal_launch_pair(ctx, n, d_u, d_keys, d_gt);     // e(U, private)
-    else b2k_internal_launch_pair(ctx, n, d_keys, d_u, d_gt);             // e(private, U)
+  uint8_t *d_key = nullptr, *d_uw = nullptr, *d_v = nullptr, *d_w = nullptr, *d_u = nullptr, *d_ok = nullptr, *d_keys = nullptr,
+          *d_gt = nullptr, *d_m = nullptr, *d_st = nullptr;
+  BlsLineCoef* tab = nullptr;
+  uint32_t* live = nullptr;
+  const int rc = host_call(ctx, [&](Carve& c) {
+    d_key = c.in(priv, KG::OUT_BYTES);
+    d_uw = c.in(u, n, UG::OUT_BYTES);
+    d_v = c.in(v, n, len);
+    d_w = c.in(w, n, len);
+    d_u = c.take<uint8_t>(n, UG::IN_BYTES);
+    d_ok = c.take<uint8_t>(n);
+    d_keys = c.take<uint8_t>(copies, KG::IN_BYTES);
+    d_gt = c.take<uint8_t>(n, 576);
+    fixed_q_layout(c, tab, live);
+    d_m = c.out(msg, n, len);
+    d_st = c.out(status, n);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    const unsigned kb = blocks_of(copies * KG::IN_BYTES, 256);
+    k_ibe_key<KG><<<kb < 1024 ? kb : 1024, 256, 0, st>>>(d_key, copies, d_keys, ctx->d_flags);
+    k_ibe_decode<UG><<<blocks_of(n, 64), 64, 0, st>>>(n, d_uw, d_u, d_ok);
     CK(cudaGetLastError());
-    ctx->launches += (ctx->pair_variant >= 16 && !(ctx->coop_max_n > 0 && n <= (size_t)ctx->coop_max_n)) ? 2 : 1;
-  }
-  k_ibe_decrypt_finish<UG><<<blocks(n, 64), 64, 0, st>>>(n, (uint32_t)len, d_gt, d_u, d_ok, d_v, d_w, d_m, d_st);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  if (len) CK(cudaMemcpyAsync(msg, d_m, n * len, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(status, d_st, n, cudaMemcpyDeviceToHost, st));
-  rc = status_finish(ctx);
+    ctx->launches += 2;
+    if (fixed_q) {
+      if (int rc = pair_fixed_q(ctx, n, d_u, d_keys, tab, live, d_gt)) return rc;
+    } else {
+      if (u_on_g1) b2k_internal_launch_pair(ctx, n, d_u, d_keys, d_gt);     // e(U, private)
+      else b2k_internal_launch_pair(ctx, n, d_keys, d_u, d_gt);             // e(private, U)
+      CK(cudaGetLastError());
+      ctx->launches += (ctx->pair_variant >= 16 && !(ctx->coop_max_n > 0 && n <= (size_t)ctx->coop_max_n)) ? 2 : 1;
+    }
+    k_ibe_decrypt_finish<UG><<<blocks_of(n, 64), 64, 0, st>>>(n, (uint32_t)len, d_gt, d_u, d_ok, d_v, d_w, d_m, d_st);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
   if (rc == B2K_ERR_POINT) ctx->err = "the private key does not decode";
   return rc;
 }
@@ -210,69 +196,48 @@ int ibe_encrypt(b2k_ctx* ctx, const uint8_t* master, const uint8_t* id, size_t i
   if (!ctx) return B2K_ERR_ARG;
   if (!dst) { dst = MG::OUT_BYTES == 48 ? DST_G2 : DST_G1; dst_len = sizeof(DST_G1) - 1; }
   if (!master || (!id && id_len) || id_len >= (size_t(1) << 31) || dst_len == 0 || dst_len > 255 || !u || n == 0 || n >= (size_t(1) << 31) ||
-      len > IBE_MAX_LEN || (len && (!msgs || !sigmas || !v || !w))) {
-    ctx->err = "bad argument (n >= 1, len <= 32, 1 <= dst_len <= 255)";
-    return B2K_ERR_ARG;
-  }
+      len > IBE_MAX_LEN || (len && (!msgs || !sigmas || !v || !w)))
+    return bad_arg(ctx, "bad argument (n >= 1, len <= 32, 1 <= dst_len <= 255)");
   CK(cudaSetDevice(ctx->device));
   using UG = MG;
-  const size_t lb = len ? len : 1;
-  int rc = arena_reserve(ctx, pad256(MG::OUT_BYTES) + pad256(MG::IN_BYTES) + pad256(id_len + 1) + pad256(8) + pad256(dst_len) +
-                                  pad256(QG::IN_BYTES) + pad256(576) + 4 * pad256(n * lb) + pad256(n * UG::OUT_BYTES) + pad256(n * 32) +
-                                  2 * pad256(n * 576) + 4096);
-  if (rc) return rc;
-  uint8_t* d_mw = arena_take<uint8_t>(ctx, MG::OUT_BYTES);
-  uint8_t* d_master = arena_take<uint8_t>(ctx, MG::IN_BYTES);
-  uint8_t* d_id = arena_take<uint8_t>(ctx, id_len + 1);
-  uint32_t* d_off = arena_take<uint32_t>(ctx, 2);
-  uint8_t* d_dst = arena_take<uint8_t>(ctx, dst_len);
-  uint8_t* d_q = arena_take<uint8_t>(ctx, QG::IN_BYTES);
-  uint8_t* d_gid = arena_take<uint8_t>(ctx, 576);
-  uint8_t* d_msg = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_sig = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_v = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_w = arena_take<uint8_t>(ctx, n * lb);
-  uint8_t* d_u = arena_take<uint8_t>(ctx, n * UG::OUT_BYTES);
-  uint8_t* d_r = arena_take<uint8_t>(ctx, n * 32);
-  uint8_t* d_gidn = arena_take<uint8_t>(ctx, n * 576);
-  uint8_t* d_gtr = arena_take<uint8_t>(ctx, n * 576);
-  if (!d_gtr) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
   const uint32_t off[2] = {0, (uint32_t)id_len};
-  CK(cudaMemcpyAsync(d_mw, master, MG::OUT_BYTES, cudaMemcpyHostToDevice, st));
-  if (id_len) CK(cudaMemcpyAsync(d_id, id, id_len, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_off, off, sizeof off, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_dst, dst, dst_len, cudaMemcpyHostToDevice, st));
-  if (len) {
-    CK(cudaMemcpyAsync(d_msg, msgs, n * len, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_sig, sigmas, n * len, cudaMemcpyHostToDevice, st));
-  }
-  k_ibe_key<MG><<<1, 64, 0, st>>>(d_mw, 1, d_master, ctx->d_flags);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  rc = QG::OUT_BYTES == 96 ? b2k_bls12381_hash_to_g2_dev(ctx, 1, d_id, d_off, d_dst, (uint32_t)dst_len, d_q)
-                           : b2k_bls12381_hash_to_g1_dev(ctx, 1, d_id, d_off, d_dst, (uint32_t)dst_len, d_q);
-  if (rc) return rc;
-  if (MG::OUT_BYTES == 48) b2k_internal_launch_pair(ctx, 1, d_master, d_q, d_gid);     // Gid = e(master, Q_id)
-  else b2k_internal_launch_pair(ctx, 1, d_q, d_master, d_gid);                         // Gid = e(Q_id, master)
-  k_ibe_encrypt<UG><<<blocks(n, 64), 64, 0, st>>>(n, (uint32_t)len, d_msg, d_sig, d_gid, d_u, d_r, d_w, d_gidn, ctx->d_flags);
-  CK(cudaGetLastError());
-  b2k_internal_launch_bls12381_gt_exp(ctx, n, d_r, d_gidn, d_gtr);
-  k_ibe_encrypt_v<<<blocks(n, 128), 128, 0, st>>>(n, (uint32_t)len, d_gtr, d_sig, d_v);
-  CK(cudaGetLastError());
-  ctx->launches += 4;
-  CK(cudaMemcpyAsync(u, d_u, n * UG::OUT_BYTES, cudaMemcpyDeviceToHost, st));
-  if (len) {
-    CK(cudaMemcpyAsync(v, d_v, n * len, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(w, d_w, n * len, cudaMemcpyDeviceToHost, st));
-  }
-  rc = status_fetch_async(ctx);
-  if (rc) return rc;
-  CK(cudaStreamSynchronize(st));
-  if (*ctx->h_flags & FLAG_IBE_H3) { ctx->err = "rejection sampling failure"; return B2K_ERR_ARG; }
-  rc = check_flags(ctx);
+  uint8_t *d_mw = nullptr, *d_id = nullptr, *d_dst = nullptr, *d_msg = nullptr, *d_sig = nullptr, *d_master = nullptr, *d_q = nullptr,
+          *d_gid = nullptr, *d_r = nullptr, *d_gidn = nullptr, *d_gtr = nullptr, *d_u = nullptr, *d_v = nullptr, *d_w = nullptr;
+  uint32_t* d_off = nullptr;
+  const int rc = host_call(ctx, [&](Carve& c) {
+    d_mw = c.in(master, MG::OUT_BYTES);
+    d_id = c.in(id, id_len);
+    d_off = c.in(off, 2);
+    d_dst = c.in(dst, dst_len);
+    d_msg = c.in(msgs, n, len);
+    d_sig = c.in(sigmas, n, len);
+    d_master = c.take<uint8_t>(MG::IN_BYTES);
+    d_q = c.take<uint8_t>(QG::IN_BYTES);
+    d_gid = c.take<uint8_t>(576);
+    d_r = c.take<uint8_t>(n, 32);
+    d_gidn = c.take<uint8_t>(n, 576);
+    d_gtr = c.take<uint8_t>(n, 576);
+    d_u = c.out(u, n, UG::OUT_BYTES);
+    d_v = c.out(v, n, len);
+    d_w = c.out(w, n, len);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_ibe_key<MG><<<1, 64, 0, st>>>(d_mw, 1, d_master, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    int rc = QG::OUT_BYTES == 96 ? b2k_bls12381_hash_to_g2_dev(ctx, 1, d_id, d_off, d_dst, (uint32_t)dst_len, d_q)
+                                 : b2k_bls12381_hash_to_g1_dev(ctx, 1, d_id, d_off, d_dst, (uint32_t)dst_len, d_q);
+    if (rc) return rc;
+    if (MG::OUT_BYTES == 48) b2k_internal_launch_pair(ctx, 1, d_master, d_q, d_gid);     // Gid = e(master, Q_id)
+    else b2k_internal_launch_pair(ctx, 1, d_q, d_master, d_gid);                         // Gid = e(Q_id, master)
+    k_ibe_encrypt<UG><<<blocks_of(n, 64), 64, 0, st>>>(n, (uint32_t)len, d_msg, d_sig, d_gid, d_u, d_r, d_w, d_gidn, ctx->d_flags);
+    CK(cudaGetLastError());
+    b2k_internal_launch_bls12381_gt_exp(ctx, n, d_r, d_gidn, d_gtr);
+    k_ibe_encrypt_v<<<blocks_of(n, 128), 128, 0, st>>>(n, (uint32_t)len, d_gtr, d_sig, d_v);
+    CK(cudaGetLastError());
+    ctx->launches += 4;
+    return B2K_OK;
+  });
   if (rc == B2K_ERR_POINT) ctx->err = "the master key does not decode";
   return rc;
 }
@@ -301,20 +266,15 @@ int b2k_bls12381_ibe_encrypt_cca_g2(b2k_ctx* ctx, const uint8_t* master, const u
 int b2k_bls12381_pair_fixed_g2(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* gt) {
   if (!ctx || !g1 || !g2 || !gt || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, pad256(n * 96) + pad256(192) + pad256(n * 576) + FIXED_Q_SCRATCH + 1024);
-  if (rc) return rc;
-  uint8_t* d1 = arena_take<uint8_t>(ctx, n * 96);
-  uint8_t* d2 = arena_take<uint8_t>(ctx, 192);
-  uint8_t* dg = arena_take<uint8_t>(ctx, n * 576);
-  cudaStream_t st = ctx->stream;
-  rc = status_begin(ctx);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d1, g1, n * 96, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d2, g2, 192, cudaMemcpyHostToDevice, st));
-  rc = pair_fixed_q(ctx, n, d1, d2, dg);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(gt, dg, n * 576, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d1 = nullptr, *d2 = nullptr, *dg = nullptr;
+  BlsLineCoef* tab = nullptr;
+  uint32_t* live = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d1 = c.in(g1, n, 96);
+    d2 = c.in(g2, 192);
+    dg = c.out(gt, n, 576);
+    fixed_q_layout(c, tab, live);
+  }, [&] { return pair_fixed_q(ctx, n, d1, d2, tab, live, dg); });
 }
 
 }  // extern "C"

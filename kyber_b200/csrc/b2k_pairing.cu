@@ -71,18 +71,12 @@ int b2k_bls12381_pair_dev(b2k_ctx* ctx, size_t n, const void* d_g1, const void* 
 int b2k_bls12381_pair(b2k_ctx* ctx, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* gt) {
   if (!ctx || !g1 || !g2 || !gt || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = b2k_arena_reserve(ctx, n * (96 + 192 + 576) + 4096);
-  if (rc) return rc;
-  uint8_t* d1 = (uint8_t*)b2k_arena_take(ctx, n * 96);
-  uint8_t* d2 = (uint8_t*)b2k_arena_take(ctx, n * 192);
-  uint8_t* dg = (uint8_t*)b2k_arena_take(ctx, n * 576);
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, ctx->stream));
-  CK(cudaMemcpyAsync(d1, g1, n * 96, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(d2, g2, n * 192, cudaMemcpyHostToDevice, ctx->stream));
-  rc = b2k_bls12381_pair_dev(ctx, n, d1, d2, dg);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(gt, dg, n * 576, cudaMemcpyDeviceToHost, ctx->stream));
-  return b2k_host::status_finish(ctx);
+  uint8_t *d1 = nullptr, *d2 = nullptr, *dg = nullptr;
+  return b2k_host::host_call(ctx, [&](b2k_host::Carve& c) {
+    d1 = c.in(g1, n, 96);
+    d2 = c.in(g2, n, 192);
+    dg = c.out(gt, n, 576);
+  }, [&] { return b2k_bls12381_pair_dev(ctx, n, d1, d2, dg); });
 }
 
 int b2k_bls12381_pairing_check_dev(b2k_ctx* ctx, size_t n, const void* a1, const void* a2, const void* b1,
@@ -99,25 +93,17 @@ int b2k_bls12381_pairing_check(b2k_ctx* ctx, size_t n, const uint8_t* a1, const 
                                const uint8_t* b2, uint8_t* ok) {
   if (!ctx || !a1 || !a2 || !b1 || !b2 || !ok || n == 0) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = b2k_arena_reserve(ctx, n * (2 * 96 + 2 * 192 + 1) + 8192);
-  if (rc) return rc;
-  uint8_t* da1 = (uint8_t*)b2k_arena_take(ctx, n * 96);
-  uint8_t* da2 = (uint8_t*)b2k_arena_take(ctx, n * 192);
-  uint8_t* db1 = (uint8_t*)b2k_arena_take(ctx, n * 96);
-  uint8_t* db2 = (uint8_t*)b2k_arena_take(ctx, n * 192);
-  uint8_t* dok = (uint8_t*)b2k_arena_take(ctx, n);
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, ctx->stream));
-  CK(cudaMemcpyAsync(da1, a1, n * 96, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(da2, a2, n * 192, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(db1, b1, n * 96, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(db2, b2, n * 192, cudaMemcpyHostToDevice, ctx->stream));
-  rc = b2k_bls12381_pairing_check_dev(ctx, n, da1, da2, db1, db2, dok);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(ok, dok, n, cudaMemcpyDeviceToHost, ctx->stream));
-  {                                          // a malformed operand already made its own check fail (ok[i] = 0): like the reference's
-    int rc2 = b2k_host::status_finish(ctx);  // ValidatePairing, the call itself reports per-element booleans, not an error
-    return rc2 == B2K_ERR_POINT ? B2K_OK : rc2;
-  }
+  uint8_t *da1 = nullptr, *da2 = nullptr, *db1 = nullptr, *db2 = nullptr, *dok = nullptr;
+  const int rc = b2k_host::host_call(ctx, [&](b2k_host::Carve& c) {
+    da1 = c.in(a1, n, 96);
+    da2 = c.in(a2, n, 192);
+    db1 = c.in(b1, n, 96);
+    db2 = c.in(b2, n, 192);
+    dok = c.out(ok, n);
+  }, [&] { return b2k_bls12381_pairing_check_dev(ctx, n, da1, da2, db1, db2, dok); });
+  // a malformed operand already made its own check fail (ok[i] = 0): like the reference's ValidatePairing, the call itself
+  // reports per-element booleans, not an error
+  return rc == B2K_ERR_POINT ? B2K_OK : rc;
 }
 
 int b2k_set_pairing_coop(b2k_ctx* ctx, int max_n) {

@@ -77,19 +77,6 @@ __global__ void __launch_bounds__(128) k_pvss_dec_verify(size_t n, const uint8_t
 
 namespace {
 
-// copy the host inputs (pointer, bytes) into the device buffers, run enqueue(), copy the status bytes back and synchronise
-template <class Fn>
-int run_staged(b2k_ctx* ctx, std::initializer_list<std::pair<uint8_t*, std::pair<const uint8_t*, size_t>>> ins, Fn&& enqueue,
-               uint8_t* status, const uint8_t* d_status, size_t n) {
-  cudaStream_t st = ctx->stream;
-  for (const auto& in : ins) CK(cudaMemcpyAsync(in.first, in.second.first, in.second.second, cudaMemcpyHostToDevice, st));
-  int rc = enqueue();
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(status, d_status, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return B2K_OK;
-}
-
 int dleq_enqueue(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint8_t* h, const uint8_t* xg, const uint8_t* xh,
                  const uint8_t* proofs, uint8_t* status) {
   k_ed_dleq_verify<<<blocks_of(n, 128), 128, 0, ctx->stream>>>(n, g, h, xg, xh, proofs, status);
@@ -115,17 +102,14 @@ int b2k_ed25519_dleq_verify(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint
   if (!ctx || !g || !h || !xg || !xh || !proofs || !status || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   uint8_t *d_g = nullptr, *d_h = nullptr, *d_xg = nullptr, *d_xh = nullptr, *d_p = nullptr, *d_st = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_g = c.take<uint8_t>(n * 32);
-    d_h = c.take<uint8_t>(n * 32);
-    d_xg = c.take<uint8_t>(n * 32);
-    d_xh = c.take<uint8_t>(n * 32);
-    d_p = c.take<uint8_t>(n * 128);
-    d_st = c.take<uint8_t>(n);
-  });
-  if (rc) return rc;
-  return run_staged(ctx, {{d_g, {g, n * 32}}, {d_h, {h, n * 32}}, {d_xg, {xg, n * 32}}, {d_xh, {xh, n * 32}}, {d_p, {proofs, n * 128}}},
-                    [&] { return dleq_enqueue(ctx, n, d_g, d_h, d_xg, d_xh, d_p, d_st); }, status, d_st, n);
+  return host_call(ctx, [&](Carve& c) {
+    d_g = c.in(g, n, 32);
+    d_h = c.in(h, n, 32);
+    d_xg = c.in(xg, n, 32);
+    d_xh = c.in(xh, n, 32);
+    d_p = c.in(proofs, n, 128);
+    d_st = c.out(status, n);
+  }, [&] { return dleq_enqueue(ctx, n, d_g, d_h, d_xg, d_xh, d_p, d_st); });
 }
 
 int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t n, const uint8_t* h, const uint8_t* commits,
@@ -140,24 +124,22 @@ int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t 
           *d_st = nullptr;
   EdNiels* d_cm = nullptr;
   uint32_t *d_bad = nullptr, *d_chal = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_h = c.take<uint8_t>(m * 32);
-    d_c = c.take<uint8_t>(mt * 32);
-    d_x = c.take<uint8_t>(mn * 32);
-    d_sh = c.take<uint8_t>(mn * 32);
-    d_v = c.take<uint8_t>(mn * 32);
-    d_p = c.take<uint8_t>(mn * 128);
-    d_cm = c.take<EdNiels>(mt);
-    d_hashed = c.take<uint8_t>(mn * 128);
-    d_bad = c.take<uint32_t>(m);
-    d_chal = c.take<uint32_t>(m * 8);
-    d_st = c.take<uint8_t>(mn);
-  });
-  if (rc) return rc;
   cudaStream_t st = ctx->stream;
   // stages, one kernel each (tools/perf_pvss.py times them by name): commitments, coms (Horner) and canonical points,
   // per-deal hash and Pick, per-share verify
-  auto enqueue = [&]() -> int {
+  return host_call(ctx, [&](Carve& c) {
+    d_h = c.in(h, m, 32);
+    d_c = c.in(commits, mt, 32);
+    d_x = c.in(x, mn, 32);
+    d_sh = c.in(sh, mn, 32);
+    d_v = c.in(v, mn, 32);
+    d_p = c.in(proofs, mn, 128);
+    d_cm = c.take<EdNiels>(mt);
+    d_hashed = c.take<uint8_t>(mn, 128);
+    d_bad = c.take<uint32_t>(m);
+    d_chal = c.take<uint32_t>(m, 8);
+    d_st = c.out(status, mn);
+  }, [&]() -> int {
     CK(cudaMemsetAsync(d_bad, 0, m * 4, st));
     k_pvss_load_commits<<<blocks_of(mt, 256), 256, 0, st>>>(mt, (uint32_t)t, d_c, d_cm, d_bad);
     k_pvss_hashed_points<<<blocks_of(mn, 128), 128, 0, st>>>((uint32_t)m, (uint32_t)t, (uint32_t)n, d_cm, d_v, d_p, d_hashed, d_bad);
@@ -166,10 +148,7 @@ int b2k_ed25519_pvss_verify_enc_shares(b2k_ctx* ctx, size_t m, size_t t, size_t 
     CK(cudaGetLastError());
     ctx->launches += 4;
     return B2K_OK;
-  };
-  return run_staged(ctx, {{d_h, {h, m * 32}}, {d_c, {commits, mt * 32}}, {d_x, {x, mn * 32}}, {d_sh, {sh, mn * 32}},
-                          {d_v, {v, mn * 32}}, {d_p, {proofs, mn * 128}}},
-                    enqueue, status, d_st, mn);
+  });
 }
 
 int b2k_ed25519_pvss_verify_dec_shares(b2k_ctx* ctx, size_t n, const uint8_t* g, const uint8_t* x, const uint8_t* enc_v,
@@ -177,23 +156,19 @@ int b2k_ed25519_pvss_verify_dec_shares(b2k_ctx* ctx, size_t n, const uint8_t* g,
   if (!ctx || !g || !x || !enc_v || !dec_v || !proofs || !status || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
   uint8_t *d_g = nullptr, *d_x = nullptr, *d_e = nullptr, *d_d = nullptr, *d_p = nullptr, *d_st = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_g = c.take<uint8_t>(32);
-    d_x = c.take<uint8_t>(n * 32);
-    d_e = c.take<uint8_t>(n * 32);
-    d_d = c.take<uint8_t>(n * 32);
-    d_p = c.take<uint8_t>(n * 128);
-    d_st = c.take<uint8_t>(n);
+  return host_call(ctx, [&](Carve& c) {
+    d_g = c.in(g, 32);
+    d_x = c.in(x, n, 32);
+    d_e = c.in(enc_v, n, 32);
+    d_d = c.in(dec_v, n, 32);
+    d_p = c.in(proofs, n, 128);
+    d_st = c.out(status, n);
+  }, [&]() -> int {
+    k_pvss_dec_verify<<<blocks_of(n, 128), 128, 0, ctx->stream>>>(n, d_g, d_x, d_e, d_d, d_p, d_st);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
   });
-  if (rc) return rc;
-  return run_staged(ctx, {{d_g, {g, 32}}, {d_x, {x, n * 32}}, {d_e, {enc_v, n * 32}}, {d_d, {dec_v, n * 32}}, {d_p, {proofs, n * 128}}},
-                    [&]() -> int {
-                      k_pvss_dec_verify<<<blocks_of(n, 128), 128, 0, ctx->stream>>>(n, d_g, d_x, d_e, d_d, d_p, d_st);
-                      CK(cudaGetLastError());
-                      ctx->launches += 1;
-                      return B2K_OK;
-                    },
-                    status, d_st, n);
 }
 
 }  // extern "C"

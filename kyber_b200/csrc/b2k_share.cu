@@ -104,7 +104,7 @@ static int recover_commit(b2k_ctx* ctx, size_t t, const uint32_t* indices, const
   });
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
+  if ((rc = status_begin(ctx))) return rc;
   CK(cudaMemcpyAsync(d_idx, indices, t * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_p, points, t * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, st));
   k_lagrange_at_zero<FR><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, d_idx, d_s, ctx->d_flags);
@@ -112,11 +112,7 @@ static int recover_commit(b2k_ctx* ctx, size_t t, const uint32_t* indices, const
   rc = msm_enqueue<CV>(ctx, s, d_s, d_p, d_o);
   if (rc) return rc;
   CK(cudaMemcpyAsync(out, d_o, CV::OUT_BYTES, cudaMemcpyDeviceToHost, st));
-  rc = status_fetch_async(ctx);
-  if (rc) return rc;
-  CK(cudaStreamSynchronize(st));
-  if (*ctx->h_flags & 4u) { ctx->err = "duplicate share index"; return B2K_ERR_ARG; }
-  return check_flags(ctx);
+  return status_finish(ctx);
 }
 
 template <class CV>
@@ -124,23 +120,22 @@ static int pubpoly_eval(b2k_ctx* ctx, size_t t, const uint8_t* commits, size_t n
   using F = typename CV::F;
   if (!ctx || !commits || !indices || !out || t == 0 || n == 0 || t >= (size_t(1) << 31) || n >= (size_t(1) << 31)) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int rc = arena_reserve(ctx, pad256(t * (size_t)CV::IN_BYTES) + pad256(t * sizeof(Affine<F>)) + pad256(n * 4) +
-                                  pad256(n * (size_t)CV::IN_BYTES) + 4096);
-  if (rc) return rc;
-  uint8_t* d_c = arena_take<uint8_t>(ctx, t * (size_t)CV::IN_BYTES);
-  auto* d_cm = arena_take<Affine<F>>(ctx, t);
-  uint32_t* d_idx = arena_take<uint32_t>(ctx, n);
-  uint8_t* d_o = arena_take<uint8_t>(ctx, n * (size_t)CV::IN_BYTES);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(d_c, commits, t * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_idx, indices, n * 4, cudaMemcpyHostToDevice, st));
-  k_load_points<CV><<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_c, d_cm, ctx->d_flags);
-  k_pubpoly_eval<CV><<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)t, d_cm, (uint32_t)n, d_idx, d_o);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  CK(cudaMemcpyAsync(out, d_o, n * (size_t)CV::IN_BYTES, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d_c = nullptr, *d_o = nullptr;
+  uint32_t* d_idx = nullptr;
+  Affine<F>* d_cm = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_c = c.in(commits, t, CV::IN_BYTES);
+    d_idx = c.in(indices, n);
+    d_cm = c.take<Affine<F>>(t);
+    d_o = c.out(out, n, CV::IN_BYTES);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_load_points<CV><<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_c, d_cm, ctx->d_flags);
+    k_pubpoly_eval<CV><<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)t, d_cm, (uint32_t)n, d_idx, d_o);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return B2K_OK;
+  });
 }
 
 template <class CV>
@@ -151,25 +146,23 @@ static int pubpoly_check(b2k_ctx* ctx, size_t m, size_t t, const uint8_t* commit
       m * n >= (size_t(1) << 31)) return B2K_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const size_t mt = m * t, mn = m * n;
-  int rc = arena_reserve(ctx, pad256(mt * (size_t)CV::IN_BYTES) + pad256(mt * sizeof(Affine<F>)) + pad256(mn * 4) +
-                                  pad256(mn * 32) + pad256(mn) + 4096);
-  if (rc) return rc;
-  uint8_t* d_c = arena_take<uint8_t>(ctx, mt * (size_t)CV::IN_BYTES);
-  auto* d_cm = arena_take<Affine<F>>(ctx, mt);
-  uint32_t* d_idx = arena_take<uint32_t>(ctx, mn);
-  uint8_t* d_s = arena_take<uint8_t>(ctx, mn * 32);
-  uint8_t* d_ok = arena_take<uint8_t>(ctx, mn);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(d_c, commits, mt * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_idx, indices, mn * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_s, shares, mn * 32, cudaMemcpyHostToDevice, st));
-  k_load_points<CV><<<(unsigned)((mt + 255) / 256), 256, 0, st>>>(mt, d_c, d_cm, ctx->d_flags);
-  k_pubpoly_check<CV><<<(unsigned)((mn + 127) / 128), 128, 0, st>>>((uint32_t)m, (uint32_t)t, d_cm, (uint32_t)n, d_idx, d_s, d_ok, ctx->use_glv);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  CK(cudaMemcpyAsync(ok, d_ok, mn, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d_c = nullptr, *d_s = nullptr, *d_ok = nullptr;
+  uint32_t* d_idx = nullptr;
+  Affine<F>* d_cm = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_c = c.in(commits, mt, CV::IN_BYTES);
+    d_idx = c.in(indices, mn);
+    d_s = c.in(shares, mn, 32);
+    d_cm = c.take<Affine<F>>(mt);
+    d_ok = c.out(ok, mn);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_load_points<CV><<<(unsigned)((mt + 255) / 256), 256, 0, st>>>(mt, d_c, d_cm, ctx->d_flags);
+    k_pubpoly_check<CV><<<(unsigned)((mn + 127) / 128), 128, 0, st>>>((uint32_t)m, (uint32_t)t, d_cm, (uint32_t)n, d_idx, d_s, d_ok, ctx->use_glv);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return B2K_OK;
+  });
 }
 
 extern "C" {

@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(128) k_lagrange_basis(uint32_t t, const uint32
     fp_mul(acc, acc, xj);
     fp_add(acc, acc, q);
   }
-  if (fp_is_zero(acc)) atomicOr(flags, 4u);                         // x_j is a double root: duplicate index
+  if (fp_is_zero(acc)) atomicOr(flags, FLAG_DUP_INDEX);                         // x_j is a double root: duplicate index
   S inv;
   fp_inv(inv, acc);
   for (uint32_t k = 0; k < t; k++) {
@@ -169,63 +169,55 @@ template <class CV, class FR>
 static int recover_pubpoly(b2k_ctx* ctx, size_t t, const uint32_t* indices, const uint8_t* points, uint8_t* commits_out) {
   using F = typename CV::F;
   using S = Fp<FR>;
-  if (!ctx || !indices || !points || !commits_out || t == 0 || t > 4096) { if (ctx) ctx->err = "bad argument (1 <= t <= 4096)"; return B2K_ERR_ARG; }
+  if (!ctx || !indices || !points || !commits_out || t == 0 || t > 4096) return bad_arg(ctx, "bad argument (1 <= t <= 4096)");
   CK(cudaSetDevice(ctx->device));
-  const size_t tt = t * t, pb = (size_t)CV::IN_BYTES;
-  int rc = arena_reserve(ctx, pad256(t * 4) + pad256(t * pb) + pad256(t * sizeof(Affine<F>)) + 2 * pad256((t + 1) * sizeof(S)) + pad256(tt * sizeof(S)) +
-                                  pad256(tt * 32) + pad256(tt * sizeof(Affine<F>)) + pad256(t * sizeof(Jac<F>)) + pad256(t * pb) + 4096);
-  if (rc) return rc;
-  uint32_t* d_idx = arena_take<uint32_t>(ctx, t);
-  uint8_t* d_p = arena_take<uint8_t>(ctx, t * pb);
-  auto* d_pm = arena_take<Affine<F>>(ctx, t);
-  S* ca = arena_take<S>(ctx, t + 1);
-  S* cb = arena_take<S>(ctx, t + 1);
-  S* rows = arena_take<S>(ctx, tt);
-  uint8_t* scal = arena_take<uint8_t>(ctx, tt * 32);
-  auto* terms = arena_take<Affine<F>>(ctx, tt);
-  auto* sums = arena_take<Jac<F>>(ctx, t);
-  uint8_t* d_o = arena_take<uint8_t>(ctx, t * pb);
-  if (!d_o) { ctx->err = "scratch arena too small"; return B2K_ERR_ARG; }
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(d_idx, indices, t * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_p, points, t * pb, cudaMemcpyHostToDevice, st));
-  k_load_points<CV><<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_p, d_pm, ctx->d_flags);
-  k_master_poly<FR><<<1, 1024, 0, st>>>((uint32_t)t, d_idx, ca, cb);
-  k_lagrange_basis<FR><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, d_idx, ca, rows, scal, ctx->d_flags);
-  k_scale_points<CV><<<(unsigned)((tt + 127) / 128), 128, 0, st>>>(tt, (uint32_t)t, scal, d_pm, terms, ctx->d_flags, ctx->use_glv);
-  k_column_sum<CV><<<(unsigned)t, 64, 0, st>>>((uint32_t)t, terms, sums);
-  k_sums_to_affine<CV><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, sums, d_o);
-  CK(cudaGetLastError());
-  ctx->launches += 6;
-  CK(cudaMemcpyAsync(commits_out, d_o, t * pb, cudaMemcpyDeviceToHost, st));
-  rc = status_fetch_async(ctx);
-  if (rc) return rc;
-  CK(cudaStreamSynchronize(st));
-  if (*ctx->h_flags & 4u) { ctx->err = "duplicate share index"; return B2K_ERR_ARG; }
-  return check_flags(ctx);
+  const size_t tt = t * t;
+  uint32_t* d_idx = nullptr;
+  uint8_t *d_p = nullptr, *scal = nullptr, *d_o = nullptr;
+  Affine<F> *d_pm = nullptr, *terms = nullptr;
+  S *ca = nullptr, *cb = nullptr, *rows = nullptr;
+  Jac<F>* sums = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_idx = c.in(indices, t);
+    d_p = c.in(points, t, CV::IN_BYTES);
+    d_pm = c.take<Affine<F>>(t);
+    ca = c.take<S>(t + 1);
+    cb = c.take<S>(t + 1);
+    rows = c.take<S>(tt);
+    scal = c.take<uint8_t>(tt, 32);
+    terms = c.take<Affine<F>>(tt);
+    sums = c.take<Jac<F>>(t);
+    d_o = c.out(commits_out, t, CV::IN_BYTES);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_load_points<CV><<<(unsigned)((t + 255) / 256), 256, 0, st>>>(t, d_p, d_pm, ctx->d_flags);
+    k_master_poly<FR><<<1, 1024, 0, st>>>((uint32_t)t, d_idx, ca, cb);
+    k_lagrange_basis<FR><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, d_idx, ca, rows, scal, ctx->d_flags);
+    k_scale_points<CV><<<(unsigned)((tt + 127) / 128), 128, 0, st>>>(tt, (uint32_t)t, scal, d_pm, terms, ctx->d_flags, ctx->use_glv);
+    k_column_sum<CV><<<(unsigned)t, 64, 0, st>>>((uint32_t)t, terms, sums);
+    k_sums_to_affine<CV><<<(unsigned)((t + 127) / 128), 128, 0, st>>>((uint32_t)t, sums, d_o);
+    CK(cudaGetLastError());
+    ctx->launches += 6;
+    return B2K_OK;
+  });
 }
 
 // PriPoly.Commit (poly.go:143-149): out[i] = scalars[i] * base (base == NULL: the group's generator), operand form
 template <class CV>
 static int commit_batch(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* base, uint8_t* out) {
-  if (!ctx || !scalars || !out || n == 0) { if (ctx) ctx->err = "bad argument"; return B2K_ERR_ARG; }
+  if (!ctx || !scalars || !out || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t pb = (size_t)CV::IN_BYTES;
-  int rc = arena_reserve(ctx, pad256(n * 32) + pad256(pb) + pad256(n * pb) + 1024);
-  if (rc) return rc;
-  uint8_t* d_s = arena_take<uint8_t>(ctx, n * 32);
-  uint8_t* d_b = arena_take<uint8_t>(ctx, pb);
-  uint8_t* d_o = arena_take<uint8_t>(ctx, n * pb);
-  cudaStream_t st = ctx->stream;
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, st));
-  CK(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, st));
-  if (base) CK(cudaMemcpyAsync(d_b, base, pb, cudaMemcpyHostToDevice, st));
-  k_commit_batch<CV><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, d_s, base ? d_b : nullptr, d_o, ctx->d_flags, ctx->use_glv);
-  CK(cudaGetLastError());
-  ctx->launches += 1;
-  CK(cudaMemcpyAsync(out, d_o, n * pb, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
+  uint8_t *d_s = nullptr, *d_b = nullptr, *d_o = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_s = c.in(scalars, n, 32);
+    d_b = c.in(base, base ? CV::IN_BYTES : 0);
+    d_o = c.out(out, n, CV::IN_BYTES);
+  }, [&]() -> int {
+    k_commit_batch<CV><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(n, d_s, base ? d_b : nullptr, d_o, ctx->d_flags, ctx->use_glv);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return B2K_OK;
+  });
 }
 
 extern "C" {

@@ -187,54 +187,47 @@ int b2k_ed25519_shuffle_verify(b2k_ctx* ctx, size_t m, size_t k, const uint8_t* 
           *d_st = nullptr;
   EdAff *d_pp = nullptr, *d_ip = nullptr, *d_gh = nullptr;
   EdExt *d_uw = nullptr, *d_part = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_p = c.take<uint8_t>(m * nitem * 32);
-    d_in = c.take<uint8_t>(4 * mk * 32);
-    if (g) d_g = c.take<uint8_t>(m * 32);
-    if (h) d_h = c.take<uint8_t>(m * 32);
-    d_zrho = c.take<uint8_t>(mk * 32);
-    d_tc = c.take<uint8_t>(m * 64);
-    d_fl = c.take<uint8_t>(m * 4);
-    d_st = c.take<uint8_t>(m);
+  // the transcript (host threads) runs while the inputs are staged and decoded on the device
+  std::vector<uint8_t> zrho(mk * 32), tc(m * 64);
+  std::thread fs([&] { b2k::shuffle_host::transcripts(m, k, proofs, proto, proto_len, zrho.data(), tc.data(), host_threads()); });
+  auto join = [&] { if (fs.joinable()) fs.join(); };
+  const int rc = host_call(ctx, [&](Carve& c) {
+    d_p = c.in(proofs, m * nitem, 32);
+    d_in = c.take<uint8_t>(4 * mk, 32);
+    const uint8_t* in[4] = {x, y, xbar, ybar};
+    for (int q = 0; q < 4; q++) c.copy_in(d_in + q * mk * 32, in[q], mk * 32);
+    if (g) d_g = c.in(g, m, 32);
+    if (h) d_h = c.in(h, m, 32);
+    d_zrho = c.take<uint8_t>(mk, 32);
+    d_tc = c.take<uint8_t>(m, 64);
+    d_fl = c.take<uint8_t>(m, 4);
+    d_st = c.out(status, m);
     d_pp = c.take<EdAff>(m * nitem);
     d_ip = c.take<EdAff>(4 * mk);
     d_gh = c.take<EdAff>(2 * m);
     d_uw = c.take<EdExt>(2 * m);
     d_part = c.take<EdExt>(2 * m * nchunk);
-  });
-  if (rc) return rc;
-  // the transcript (host threads) runs while the inputs are staged and decoded on the device
-  std::vector<uint8_t> zrho(mk * 32), tc(m * 64);
-  std::thread fs([&] { b2k::shuffle_host::transcripts(m, k, proofs, proto, proto_len, zrho.data(), tc.data(), host_threads()); });
-  cudaStream_t st = ctx->stream;
-  auto stage = [&]() -> int {
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
     CK(cudaMemsetAsync(d_fl, 0, m * 4, st));
-    CK(cudaMemcpyAsync(d_p, proofs, m * nitem * 32, cudaMemcpyHostToDevice, st));
-    const uint8_t* in[4] = {x, y, xbar, ybar};
-    for (int q = 0; q < 4; q++) CK(cudaMemcpyAsync(d_in + q * mk * 32, in[q], mk * 32, cudaMemcpyHostToDevice, st));
-    if (g) CK(cudaMemcpyAsync(d_g, g, m * 32, cudaMemcpyHostToDevice, st));
-    if (h) CK(cudaMemcpyAsync(d_h, h, m * 32, cudaMemcpyHostToDevice, st));
     k_shuffle_decode<<<blocks_of(m * nitem + 4 * mk + 2 * m, 256), 256, 0, st>>>((uint32_t)m, (uint32_t)k, d_p, d_in, d_g, d_h,
                                                                                  d_pp, d_ip, d_gh, d_fl);
     CK(cudaGetLastError());
+    join();
+    CK(cudaMemcpyAsync(d_zrho, zrho.data(), mk * 32, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tc, tc.data(), m * 64, cudaMemcpyHostToDevice, st));
+    k_shuffle_uw<<<blocks_of(2 * m, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, d_pp, d_gh, d_tc, d_uw);
+    k_shuffle_thver<<<blocks_of(2 * mk, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, d_p, d_pp, d_gh, d_uw, d_tc, d_fl);
+    k_shuffle_pair_terms<<<(unsigned)(m * nchunk), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, (uint32_t)nchunk, d_p, d_pp, d_ip,
+                                                                      d_zrho, d_fl, d_part);
+    k_shuffle_resolve<<<(unsigned)m, SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, (uint32_t)nchunk, d_p, d_pp, d_gh, d_part, d_fl,
+                                                       d_st);
+    CK(cudaGetLastError());
+    ctx->launches += 5;
     return B2K_OK;
-  };
-  rc = stage();
-  fs.join();
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(d_zrho, zrho.data(), mk * 32, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_tc, tc.data(), m * 64, cudaMemcpyHostToDevice, st));
-  k_shuffle_uw<<<blocks_of(2 * m, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, d_pp, d_gh, d_tc, d_uw);
-  k_shuffle_thver<<<blocks_of(2 * mk, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, d_p, d_pp, d_gh, d_uw, d_tc, d_fl);
-  k_shuffle_pair_terms<<<(unsigned)(m * nchunk), SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, (uint32_t)nchunk, d_p, d_pp, d_ip,
-                                                                    d_zrho, d_fl, d_part);
-  k_shuffle_resolve<<<(unsigned)m, SHUF_BS, 0, st>>>((uint32_t)m, (uint32_t)k, (uint32_t)nchunk, d_p, d_pp, d_gh, d_part, d_fl,
-                                                     d_st);
-  CK(cudaGetLastError());
-  ctx->launches += 5;
-  CK(cudaMemcpyAsync(status, d_st, m, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return B2K_OK;
+  });
+  join();   // every failure path, a failed reservation included
+  return rc;
 }
 
 int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, const uint8_t* x, const uint8_t* y,
@@ -247,25 +240,23 @@ int b2k_ed25519_shuffle_sequence_verifiable(b2k_ctx* ctx, size_t nq, size_t k, c
   const size_t n = nq * k;
   uint8_t *d_in = nullptr, *d_e = nullptr, *d_out = nullptr;
   EdAff* d_pts = nullptr;
-  int rc = arena_carve(ctx, [&](Carve& c) {
-    d_in = c.take<uint8_t>(4 * n * 32);
-    d_e = c.take<uint8_t>(nq * 32);
-    d_out = c.take<uint8_t>(4 * k * 32);
+  return host_call(ctx, [&](Carve& c) {
+    d_in = c.take<uint8_t>(4 * n, 32);
+    const uint8_t* in[4] = {x, y, xbar, ybar};
+    for (int q = 0; q < 4; q++) c.copy_in(d_in + q * n * 32, in[q], n * 32);
+    d_e = c.in(e, nq, 32);
+    d_out = c.take<uint8_t>(4 * k, 32);
+    uint8_t* outs[4] = {x_up, y_up, x_down, y_down};
+    for (int q = 0; q < 4; q++) c.copy_out(outs[q], d_out + q * k * 32, k * 32);
     d_pts = c.take<EdAff>(4 * n);
+  }, [&]() -> int {
+    cudaStream_t st = ctx->stream;
+    k_shuffle_seq_decode<<<blocks_of(4 * n, 256), 256, 0, st>>>(4 * n, d_in, d_pts, ctx->d_flags);
+    k_shuffle_seq_terms<<<blocks_of(4 * k, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)nq, (uint32_t)k, d_pts, d_e, d_out);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return B2K_OK;
   });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  if ((rc = status_begin(ctx))) return rc;
-  const uint8_t* in[4] = {x, y, xbar, ybar};
-  for (int q = 0; q < 4; q++) CK(cudaMemcpyAsync(d_in + q * n * 32, in[q], n * 32, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_e, e, nq * 32, cudaMemcpyHostToDevice, st));
-  k_shuffle_seq_decode<<<blocks_of(4 * n, 256), 256, 0, st>>>(4 * n, d_in, d_pts, ctx->d_flags);
-  k_shuffle_seq_terms<<<blocks_of(4 * k, SHUF_BS), SHUF_BS, 0, st>>>((uint32_t)nq, (uint32_t)k, d_pts, d_e, d_out);
-  CK(cudaGetLastError());
-  ctx->launches += 2;
-  uint8_t* outs[4] = {x_up, y_up, x_down, y_down};
-  for (int q = 0; q < 4; q++) CK(cudaMemcpyAsync(outs[q], d_out + q * k * 32, k * 32, cudaMemcpyDeviceToHost, st));
-  return status_finish(ctx);
 }
 
 }  // extern "C"

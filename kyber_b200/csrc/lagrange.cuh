@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(128) k_lagrange_at_zero(uint32_t t, const uint
                                                           uint8_t* __restrict__ scalars, uint32_t* flags) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= t) return;
-  if (!lagrange_at_zero<FR, LE>(i, t, idx, scalars + 32 * (size_t)i)) atomicOr(flags, 4u);
+  if (!lagrange_at_zero<FR, LE>(i, t, idx, scalars + 32 * (size_t)i)) atomicOr(flags, FLAG_DUP_INDEX);
 }
 #endif
 

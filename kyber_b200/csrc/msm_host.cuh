@@ -608,7 +608,7 @@ inline cudaStream_t copy_stream(b2k_ctx* ctx) {
 }
 
 // Host-buffer MSM.  wait = false: everything (H2D copies, pipeline, D2H of the result and of the status word) is only
-// ENQUEUED on the context's stream; the caller collects the status with msm_wait() (b2k_wait).  With page-locked host
+// ENQUEUED on the context's stream; the caller collects the status with b2k_wait.  With page-locked host
 // buffers the copies of one context overlap the kernels of another: two contexts alternate to keep PCIe and the SMs busy.
 template <class CV>
 int msm_host(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* points, uint8_t* out, int affine_out = 0, bool wait = true) {
@@ -652,17 +652,6 @@ int msm_host(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* poin
   return status_finish(ctx);
 }
 
-// Also the status query of the *_dev entry points, which only enqueue: the device status word (scalar range, malformed
-// point) is sticky across them, fetched and cleared here.
-inline int msm_wait(b2k_ctx* ctx) {
-  if (!ctx) return B2K_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  CK(cudaMemcpyAsync(ctx->h_flags, ctx->d_flags, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return check_flags(ctx);
-}
-
 template <class CV, bool AFF>
 int mul_batch_dev(b2k_ctx* ctx, size_t n, const void* d_scalars, const void* d_points, void* d_out) {
   if (!ctx || !d_scalars || !d_points || !d_out || n == 0) {
@@ -683,26 +672,14 @@ int mul_batch_dev(b2k_ctx* ctx, size_t n, const void* d_scalars, const void* d_p
 
 template <class CV, bool AFF>
 int mul_batch_host(b2k_ctx* ctx, size_t n, const uint8_t* scalars, const uint8_t* points, uint8_t* out) {
-  if (!ctx || !scalars || !points || !out || n == 0) {
-    if (ctx) ctx->err = "bad argument";
-    return B2K_ERR_ARG;
-  }
+  if (!ctx || !scalars || !points || !out || n == 0) return bad_arg(ctx, "bad argument");
   CK(cudaSetDevice(ctx->device));
-  const size_t ob = AFF ? (size_t)CV::IN_BYTES : (size_t)CV::OUT_BYTES;
-  size_t bytes = pad256(n * 32) + pad256(n * (size_t)CV::IN_BYTES) + pad256(n * ob) + 1024;
-  int rc = arena_reserve(ctx, bytes);
-  if (rc) return rc;
-  auto* d_s = arena_take<uint8_t>(ctx, n * 32);
-  auto* d_p = arena_take<uint8_t>(ctx, n * (size_t)CV::IN_BYTES);
-  auto* d_o = arena_take<uint8_t>(ctx, n * ob);
-  CK(cudaMemsetAsync(ctx->d_flags, 0, 4, ctx->stream));
-  CK(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(d_p, points, n * (size_t)CV::IN_BYTES, cudaMemcpyHostToDevice, ctx->stream));
-  rc = mul_batch_dev<CV, AFF>(ctx, n, d_s, d_p, d_o);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(out, d_o, n * ob, cudaMemcpyDeviceToHost, ctx->stream));
-  return status_finish(ctx);
+  uint8_t *d_s = nullptr, *d_p = nullptr, *d_o = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_s = c.in(scalars, n, 32);
+    d_p = c.in(points, n, CV::IN_BYTES);
+    d_o = c.out(out, n, AFF ? CV::IN_BYTES : CV::OUT_BYTES);
+  }, [&] { return mul_batch_dev<CV, AFF>(ctx, n, d_s, d_p, d_o); });
 }
-
 
 }  // namespace b2k_host
