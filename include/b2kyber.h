@@ -694,6 +694,64 @@ int b2k_bn256_hash_g1_dev(b2k_ctx* ctx, size_t n, const void* d_msgs, const void
 int b2k_bdn_coefficients(size_t n, const uint8_t* pubs /*[n][pub_len] MarshalBinary bytes*/, size_t pub_len, int add_one,
                          uint8_t* out /*[n][32] BE*/);
 
+/* ---- sign/bdn: masked aggregation and batch verification ----------------------------------------------------------------
+ * The verifier's workload: many aggregate signatures over ONE roster, each with its own participation mask.  Three key groups:
+ *   bls12381_g2  bdn.NewSchemeOnG1 (keys on G2, signatures on G1): keys 96 B compressed, terms 192 B operand form
+ *   bls12381_g1  bdn.NewSchemeOnG2 (keys on G1, signatures on G2): keys 48 B compressed, terms 96 B operand form
+ *   bn256_g2     bdn.NewSchemeOnG1(bn256.NewSuite()): keys and terms 128 B (bn256 has no hash onto G2: no second scheme)
+ * Terms (NewMask, sign/bdn/mask.go:34-64): terms[i] = (c_i + 1) PK_i, with c_i = b2k_bdn_coefficients over the keys'
+ *   MarshalBinary bytes -- the input bytes for BLS12-381, the canonical re-encoding (coordinates reduced mod p) for bn256,
+ *   whose Unmarshal does not range-check.  Keys decode like UnmarshalBinary (BLS12-381: b2k_bls12381_g{1,2}_decompress,
+ *   subgroup check included; bn256: b2k_bn256_g2_unmarshal_check); a key that does not decode -> B2K_ERR_POINT.
+ *   Compute them once per roster.
+ * Aggregate keys (AggregatePublicKeys, bdn.go:166-181, once per mask): out[k] = sum of terms[i] over the bits i < n set in
+ *   masks[k] (bit i of byte i/8, least significant bit first: mask.go:88-97); bits at positions >= n are ignored; an empty mask
+ *   gives infinity (all zeros).  Masks have a fixed stride of (n + 7) / 8 bytes, so the reference's "mismatching mask lengths"
+ *   is the caller's check.  A pure sum of cached terms: no scalar multiplication.  Terms are re-validated like every operand
+ *   (canonical coordinates where the curve's Unmarshal checks them, the curve equation): a violation -> B2K_ERR_POINT.
+ * Verification (bls.Verify under each aggregate key, sign/bls/bls.go:82-96): status[k] in the reference's order
+ *   B2K_BDN_SIG      the signature does not decode: "bls: unmarshalling signature point"
+ *   B2K_BDN_INVALID  the pairing equation fails: "bls: invalid signature"
+ *   msgs/offsets as in b2k_bls12381_verify_g1sig (offsets[m+1]); 0 < dst_len <= 255; bn256 hashes like b2k_bn256_hash_to_g1
+ *   (try-and-increment, no dst).  Bad signature data is never a call error; an empty mask with the infinity signature is OK,
+ *   as in the reference (e(H(m), O) = e(O, B) = 1).
+ * B2K_ERR_ARG: a null pointer, n == 0 or m == 0, n above B2K_BDN_MAX_N, m above B2K_BDN_MAX_M, dst_len out of range, decreasing
+ *   offsets (host forms).  The *_dev forms take device pointers and only enqueue; B2K_ERR_POINT then arrives at b2k_wait.
+ * Not here: AggregateSignatures (the aggregator's side, one *_msm call each) and sign.Policy (the caller pop-counts its own
+ * mask bytes).
+ *   replaces: bdn.AggregatePublicKeys + bdn.Verify called once per aggregate signature */
+#define B2K_BDN_MAX_N ((size_t)1 << 20)
+#define B2K_BDN_MAX_M ((size_t)1 << 20)
+enum { B2K_BDN_OK = 0, B2K_BDN_SIG = 1, B2K_BDN_INVALID = 2 };
+int b2k_bls12381_g2_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][96]*/, uint8_t* terms /*[n][192]*/);
+int b2k_bls12381_g1_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][48]*/, uint8_t* terms /*[n][96]*/);
+int b2k_bn256_g2_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][128]*/, uint8_t* terms /*[n][128]*/);
+int b2k_bls12381_g2_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][192]*/, size_t m,
+                                       const uint8_t* masks /*[m][(n+7)/8]*/, uint8_t* out /*[m][192]*/);
+int b2k_bls12381_g2_bdn_aggregate_keys_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks,
+                                           void* d_out);
+int b2k_bls12381_g1_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][96]*/, size_t m,
+                                       const uint8_t* masks /*[m][(n+7)/8]*/, uint8_t* out /*[m][96]*/);
+int b2k_bls12381_g1_bdn_aggregate_keys_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks,
+                                           void* d_out);
+int b2k_bn256_g2_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][128]*/, size_t m,
+                                    const uint8_t* masks /*[m][(n+7)/8]*/, uint8_t* out /*[m][128]*/);
+int b2k_bls12381_bdn_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][192]*/, size_t m,
+                                  const uint8_t* masks /*[m][(n+7)/8]*/, const uint8_t* msgs, const uint32_t* offsets /*[m+1]*/,
+                                  const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs /*[m][48]*/, uint8_t* status /*[m]*/);
+int b2k_bls12381_bdn_verify_g1sig_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks,
+                                      const void* d_msgs, const void* d_offsets, const void* d_dst, uint32_t dst_len,
+                                      const void* d_sigs, void* d_status);
+int b2k_bls12381_bdn_verify_g2sig(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][96]*/, size_t m,
+                                  const uint8_t* masks /*[m][(n+7)/8]*/, const uint8_t* msgs, const uint32_t* offsets /*[m+1]*/,
+                                  const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs /*[m][96]*/, uint8_t* status /*[m]*/);
+int b2k_bls12381_bdn_verify_g2sig_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks,
+                                      const void* d_msgs, const void* d_offsets, const void* d_dst, uint32_t dst_len,
+                                      const void* d_sigs, void* d_status);
+int b2k_bn256_bdn_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n][128]*/, size_t m,
+                               const uint8_t* masks /*[m][(n+7)/8]*/, const uint8_t* msgs, const uint32_t* offsets /*[m+1]*/,
+                               const uint8_t* sigs /*[m][64]*/, uint8_t* status /*[m]*/);
+
 #ifdef __cplusplus
 }
 #endif

@@ -428,6 +428,48 @@ class Engine:
             raise ValueError("b2k_bdn_coefficients: rc=%d" % rc)
         return out.raw
 
+    # -- sign/bdn: a roster's terms once, then aggregate keys / verification for many masks ----------------------------------
+    # key group -> the scheme whose signatures it verifies, that scheme's signature bytes and its default domain separation tag
+    # (the signature group's, kilic/g1.go:17 and g2.go:18; bn256 hashes without one)
+    BDN_SCHEMES = {"bls12381_g2": ("bls12381_bdn_verify_g1sig", 48, b"BLS_SIG_BLS12381G1_XMD:SHA-256_SSWU_RO_NUL_"),
+                   "bls12381_g1": ("bls12381_bdn_verify_g2sig", 96, b"BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_NUL_"),
+                   "bn256_g2": ("bn256_bdn_verify_g1sig", 64, None)}
+
+    def bdn_terms(self, group: str, pubs: bytes) -> bytes:
+        """NewMask's terms (c_i + 1) PK_i of a roster: group in BDN_SCHEMES, pubs [n][MarshalBinary] -> [n][operand]"""
+        operand, wire = self.POINT_BYTES[group]
+        n = len(pubs) // wire
+        assert len(pubs) == n * wire
+        return self._call(f"b2k_{group}_bdn_terms", n, pubs, out=n * operand)
+
+    def bdn_aggregate_keys(self, group: str, terms: bytes, masks) -> bytes:
+        """AggregatePublicKeys for every mask (list of (n + 7) / 8 mask bytes) -> [m][operand]"""
+        operand = self.POINT_BYTES[group][0]
+        n = len(terms) // operand
+        assert masks and all(len(k) == (n + 7) // 8 for k in masks)
+        return self._call(f"b2k_{group}_bdn_aggregate_keys", n, terms, len(masks), b"".join(masks), out=len(masks) * operand)
+
+    def bdn_aggregate_keys_dev(self, group: str, n: int, d_terms: int, m: int, d_masks: int, d_out: int):
+        self._call(f"b2k_{group}_bdn_aggregate_keys_dev", n, d_terms, m, d_masks, d_out)
+
+    def bdn_verify(self, group: str, terms: bytes, masks, msgs, sigs: bytes, dst: bytes = None) -> bytes:
+        """bls.Verify under each mask's aggregate key -> statuses [m] (B2K_BDN_OK / _SIG / _INVALID).  dst: BLS12-381 only, the
+        signature group's default when left out"""
+        name, sig_bytes, default_dst = self.BDN_SCHEMES[group]
+        n, m = len(terms) // self.POINT_BYTES[group][0], len(masks)
+        assert len(msgs) == m and len(sigs) == sig_bytes * m and all(len(k) == (n + 7) // 8 for k in masks)
+        blob, offs = self._pack_msgs(msgs)
+        if group == "bn256_g2":
+            if dst is not None:
+                raise ValueError("bn256 hashes with try-and-increment: it takes no dst")
+            return self._call(f"b2k_{name}", n, terms, m, b"".join(masks), blob, offs, sigs, out=m)
+        dst = default_dst if dst is None else dst
+        return self._call(f"b2k_{name}", n, terms, m, b"".join(masks), blob, offs, dst, len(dst), sigs, out=m)
+
+    def bdn_verify_dev(self, group: str, n: int, d_terms: int, m: int, d_masks: int, d_msgs: int, d_offsets: int, d_dst: int,
+                       dst_len: int, d_sigs: int, d_status: int):
+        self._call(f"b2k_{self.BDN_SCHEMES[group][0]}_dev", n, d_terms, m, d_masks, d_msgs, d_offsets, d_dst, dst_len, d_sigs, d_status)
+
     # -- share/poly: RecoverCommit, RecoverPubPoly, PubPoly.Eval / Check, PriPoly.Commit ---------------------------------------
     def _recover_commit(self, group: str, indices, points: bytes) -> bytes:
         operand, result = self.POINT_BYTES[group]

@@ -7,13 +7,20 @@
 // The absorb phase is one sequential hash chain over n * pub_len bytes: inherently serial, it stays on the host here as
 // in the reference (it is <1% of the curve work it feeds: the MSM over (c_i + 1, S_i) / (c_i + 1, PK_i) on the device).
 // The squeeze phase (BLAKE2X: one independent compression per 32 output bytes) is spread over host threads.
-// No device work, no context needed.
+// The coefficients need no device work and no context.
+//
+// The device half (bdn.cuh drives the bodies): the roster's terms (NewMask, mask.go:34-64) through the existing decoders and
+// Point.Mul batches, and AggregatePublicKeys (bdn.go:166-181) for many masks at once as masked sums of those terms.
 #include <cstdint>
 #include <cstring>
 #include <thread>
 #include <vector>
 
 #include "../../include/b2kyber.h"
+#define B2K_FP2_BYREF 1   // Fp2 products out of line by reference (tower.cuh), as in the G2 MSM of b2k_g2.cu: the G2 bodies hold whole XYZZ points
+#include "codec.cuh"
+#include "bn256.cuh"
+#include "bdn.cuh"
 
 namespace {
 
@@ -135,3 +142,257 @@ extern "C" int b2k_bdn_coefficients(size_t n, const uint8_t* pubs, size_t pub_le
   }
   return B2K_OK;
 }
+
+// ---- the device half ------------------------------------------------------------------------------------------------------
+namespace b2k {
+
+constexpr unsigned BDN_BLOCK = 64;   // two warps per block in the masked sum
+
+// operand bytes -> Montgomery affine in scratch, re-validated like every operand (FLAG_POINT, the term counts as infinity)
+template <class CV>
+__global__ void __launch_bounds__(128) k_bdn_load(size_t n, const uint8_t* __restrict__ wire, Affine<typename CV::F>* __restrict__ terms,
+                                                  uint32_t* flags) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  Affine<typename CV::F> a;
+  if (!load_checked<CV>(a, wire + (size_t)CV::IN_BYTES * i)) atomicOr(flags, FLAG_POINT);
+  terms[i] = a;
+}
+
+__global__ void __launch_bounds__(128) k_bdn_complement(size_t m, uint32_t n, const uint8_t* __restrict__ masks, size_t stride,
+                                                        uint8_t* __restrict__ comp) {
+  const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < m) comp[k] = bdn_complement(masks + k * stride, stride, n) ? 1 : 0;
+}
+
+// part[k nslices + s] = the masked sum of slice s of mask k: one warp per (mask, slice), lane l walks mask word 32 s + l, then the
+// lanes' sums meet in a tree through shared memory (the points stay in memory: see bdn_add).
+// masks == nullptr: the all-ones mask (m = 1), i.e. the slices of the roster total.
+template <class CV>
+__global__ void __launch_bounds__(BDN_BLOCK) k_bdn_masked_sum(size_t m, uint32_t n, uint32_t nslices, const uint8_t* __restrict__ masks,
+                                                              size_t stride, const uint8_t* __restrict__ comp,
+                                                              const Affine<typename CV::F>* __restrict__ terms, Xyzz<typename CV::F>* __restrict__ part) {
+  using X = Xyzz<typename CV::F>;
+  __shared__ X lane_sum[BDN_BLOCK];
+  const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  if (warp >= m * nslices) return;                     // whole warps only: blockDim is a multiple of 32
+  const size_t k = warp / nslices;
+  const uint32_t w = (uint32_t)(warp % nslices) * 32 + lane;
+  const uint32_t bits = bdn_lane_bits(masks ? masks + k * stride : nullptr, stride, n, w, comp && comp[k]);
+  X& acc = lane_sum[threadIdx.x];
+  xyzz_set_inf(acc);
+  bdn_walk(acc, bits, terms, 32 * w);
+  __syncwarp();
+#pragma unroll 1
+  for (uint32_t d = 16; d > 0; d >>= 1) {
+    if (lane < d) bdn_add(acc, acc, lane_sum[threadIdx.x + d]);
+    __syncwarp();
+  }
+  if (lane == 0) part[warp] = acc;
+}
+
+// total[nslices] = the roster total from its slice partials total[0 .. nslices)
+template <class CV>
+__global__ void k_bdn_total(uint32_t nslices, Xyzz<typename CV::F>* total) {
+  if (threadIdx.x || blockIdx.x) return;
+  Xyzz<typename CV::F> r;
+  bdn_combine(r, total, nslices);
+  total[nslices] = r;
+}
+
+// out + k out_stride = mask k's aggregate key in operand form
+template <class CV>
+__global__ void __launch_bounds__(64) k_bdn_finish(size_t m, uint32_t nslices, const Xyzz<typename CV::F>* __restrict__ part,
+                                                   const uint8_t* __restrict__ comp, const Xyzz<typename CV::F>* __restrict__ total,
+                                                   uint8_t* __restrict__ out, size_t out_stride) {
+  const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= m) return;
+  Affine<typename CV::F> r;
+  bdn_finish(r, part + k * nslices, nslices, comp[k] != 0, *total);
+  CV::store_affine(out + k * out_stride, r);
+}
+
+// FLAG_POINT when a roster key did not decode (NewMask only ever sees decoded points)
+__global__ void k_bdn_require(size_t n, const uint8_t* __restrict__ ok, uint32_t* flags) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && !ok[i]) atomicOr(flags, FLAG_POINT);
+}
+
+__global__ void k_bdn_status(size_t m, const uint8_t* __restrict__ sig_ok, const uint8_t* __restrict__ pair_ok,
+                             uint8_t* __restrict__ status) {
+  const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < m) status[k] = !sig_ok[k] ? B2K_BDN_SIG : (pair_ok[k] ? B2K_BDN_OK : B2K_BDN_INVALID);
+}
+
+}  // namespace b2k
+
+namespace b2k_host {
+
+int bdn_args(b2k_ctx* ctx, size_t n, size_t m) {
+  if (n == 0 || m == 0 || n > B2K_BDN_MAX_N || m > B2K_BDN_MAX_M) return bad_arg(ctx, "bdn: n and m must be in 1..2^20");
+  return B2K_OK;
+}
+
+namespace {
+
+template <class CV>
+void layout_of(Carve& c, BdnScratch& s, size_t n, size_t m) {
+  using F = typename CV::F;
+  s.nslices = (n + BDN_SLICE - 1) / BDN_SLICE;
+  s.terms = c.take<Affine<F>>(n);
+  s.comp = c.take<uint8_t>(m);
+  s.part = c.take<Xyzz<F>>(m, s.nslices);
+  s.total = c.take<Xyzz<F>>(s.nslices + 1);
+}
+
+template <class CV>
+int aggregate_enqueue(b2k_ctx* ctx, const BdnScratch& s, size_t n, const uint8_t* d_terms, size_t m, const uint8_t* d_masks,
+                      uint8_t* d_out, size_t out_stride) {
+  using F = typename CV::F;
+  cudaStream_t st = ctx->stream;
+  const size_t stride = (n + 7) / 8;
+  const uint32_t ns = (uint32_t)s.nslices;
+  auto* terms = static_cast<Affine<F>*>(s.terms);
+  auto* part = static_cast<Xyzz<F>*>(s.part);
+  auto* total = static_cast<Xyzz<F>*>(s.total);
+  k_bdn_load<CV><<<blocks_of(n, 128), 128, 0, st>>>(n, d_terms, terms, ctx->d_flags);
+  k_bdn_masked_sum<CV><<<blocks_of(32 * (size_t)ns, BDN_BLOCK), BDN_BLOCK, 0, st>>>(1, (uint32_t)n, ns, nullptr, stride, nullptr, terms, total);
+  k_bdn_total<CV><<<1, 32, 0, st>>>(ns, total);
+  k_bdn_complement<<<blocks_of(m, 128), 128, 0, st>>>(m, (uint32_t)n, d_masks, stride, s.comp);
+  k_bdn_masked_sum<CV><<<blocks_of(32 * m * ns, BDN_BLOCK), BDN_BLOCK, 0, st>>>(m, (uint32_t)n, ns, d_masks, stride, s.comp, terms, part);
+  k_bdn_finish<CV><<<blocks_of(m, 64), 64, 0, st>>>(m, ns, part, s.comp, total + ns, d_out, out_stride);
+  CK(cudaGetLastError());
+  ctx->launches += 6;
+  return B2K_OK;
+}
+
+}  // namespace
+
+void bdn_layout(Carve& c, BdnScratch& s, BdnGroup g, size_t n, size_t m) {
+  if (g == BDN_BLS_G2) layout_of<Bls381G2>(c, s, n, m);
+  else if (g == BDN_BLS_G1) layout_of<Bls381G1>(c, s, n, m);
+  else layout_of<Bn256G2>(c, s, n, m);
+}
+
+int bdn_aggregate_enqueue(b2k_ctx* ctx, BdnGroup g, const BdnScratch& s, size_t n, const uint8_t* d_terms, size_t m,
+                          const uint8_t* d_masks, uint8_t* d_out, size_t out_stride) {
+  if (g == BDN_BLS_G2) return aggregate_enqueue<Bls381G2>(ctx, s, n, d_terms, m, d_masks, d_out, out_stride);
+  if (g == BDN_BLS_G1) return aggregate_enqueue<Bls381G1>(ctx, s, n, d_terms, m, d_masks, d_out, out_stride);
+  return aggregate_enqueue<Bn256G2>(ctx, s, n, d_terms, m, d_masks, d_out, out_stride);
+}
+
+int bdn_status_enqueue(b2k_ctx* ctx, size_t m, const uint8_t* d_sig_ok, const uint8_t* d_pair_ok, uint8_t* d_status) {
+  k_bdn_status<<<blocks_of(m, 256), 256, 0, ctx->stream>>>(m, d_sig_ok, d_pair_ok, d_status);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return B2K_OK;
+}
+
+}  // namespace b2k_host
+
+namespace {
+using namespace b2k_host;
+
+constexpr size_t operand_bytes(BdnGroup g) { return g == BDN_BLS_G2 ? 192 : g == BDN_BLS_G1 ? 96 : 128; }
+
+int aggregate_host(b2k_ctx* ctx, BdnGroup g, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, uint8_t* out) {
+  if (!ctx || !terms || !masks || !out) return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, m)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  const size_t ob = operand_bytes(g);
+  BdnScratch s;
+  uint8_t *d_terms = nullptr, *d_masks = nullptr, *d_out = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_terms = c.in(terms, n, ob);
+    d_masks = c.in(masks, m, (n + 7) / 8);
+    d_out = c.out(out, m, ob);
+    bdn_layout(c, s, g, n, m);
+  }, [&] { return bdn_aggregate_enqueue(ctx, g, s, n, d_terms, m, d_masks, d_out, ob); });
+}
+
+int aggregate_dev(b2k_ctx* ctx, BdnGroup g, size_t n, const void* d_terms, size_t m, const void* d_masks, void* d_out) {
+  if (!ctx || !d_terms || !d_masks || !d_out) return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, m)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  BdnScratch s;
+  if (int rc = arena_carve(ctx, [&](Carve& c) { bdn_layout(c, s, g, n, m); })) return rc;
+  return bdn_aggregate_enqueue(ctx, g, s, n, (const uint8_t*)d_terms, m, (const uint8_t*)d_masks, (uint8_t*)d_out, operand_bytes(g));
+}
+
+// BLS12-381 terms: coefficients over the input (= MarshalBinary) bytes on the host, then UnmarshalBinary and Point.Mul on the device
+using DevCall = int (*)(b2k_ctx*, size_t, const void*, const void*, void*);
+int bls_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs, uint8_t* terms, size_t wire, size_t operand,
+              int (*decompress)(b2k_ctx*, size_t, const void*, void*, void*), DevCall mul) {
+  if (!ctx || !pubs || !terms) return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, 1)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  std::vector<uint8_t> fac(32 * n);
+  if (int rc = b2k_bdn_coefficients(n, pubs, wire, 1, fac.data())) return rc;
+  uint8_t *d_pub = nullptr, *d_fac = nullptr, *d_dec = nullptr, *d_ok = nullptr, *d_out = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_pub = c.in(pubs, n, wire);
+    d_fac = c.in(fac.data(), n, 32);
+    d_dec = c.take<uint8_t>(n, operand);
+    d_ok = c.take<uint8_t>(n);
+    d_out = c.out(terms, n, operand);
+  }, [&]() -> int {
+    if (int rc = decompress(ctx, n, d_pub, d_dec, d_ok)) return rc;
+    k_bdn_require<<<blocks_of(n, 256), 256, 0, ctx->stream>>>(n, d_ok, ctx->d_flags);
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    return mul(ctx, n, d_fac, d_dec, d_out);
+  });
+}
+
+// bn256 p, big-endian: Unmarshal reduces every coordinate below 2^256 < 2p by at most one subtraction (gfp.go:115-122)
+constexpr uint8_t BN256_P[32] = {0x8f, 0xb5, 0x01, 0xe3, 0x4a, 0xa3, 0x87, 0xf9, 0xaa, 0x6f, 0xec, 0xb8, 0x61, 0x84, 0xdc, 0x21,
+                                 0xee, 0x5b, 0x88, 0xd1, 0x20, 0xb5, 0xb5, 0x9e, 0x18, 0x5c, 0xac, 0x6c, 0x5e, 0x08, 0x96, 0x67};
+void bn256_reduce32(uint8_t* v) {
+  if (std::memcmp(v, BN256_P, 32) < 0) return;      // big-endian bytes compare as numbers
+  int borrow = 0;
+  for (int k = 31; k >= 0; k--) {
+    const int d = (int)v[k] - BN256_P[k] - borrow;
+    borrow = d < 0;
+    v[k] = (uint8_t)(d + (borrow ? 256 : 0));
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2k_bls12381_g2_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs, uint8_t* terms) {
+  return bls_terms(ctx, n, pubs, terms, 96, 192, b2k_bls12381_g2_decompress_dev, b2k_bls12381_g2_mul_batch_affine_dev);
+}
+int b2k_bls12381_g1_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs, uint8_t* terms) {
+  return bls_terms(ctx, n, pubs, terms, 48, 96, b2k_bls12381_g1_decompress_dev, b2k_bls12381_g1_mul_batch_affine_dev);
+}
+// bn256: the coefficients hash the canonical re-encoding (MarshalBinary of the decoded key); the Point.Mul batch re-checks the
+// twist equation, which is all bn256's Unmarshal checks (pairing/bn256/point.go:469-506)
+int b2k_bn256_g2_bdn_terms(b2k_ctx* ctx, size_t n, const uint8_t* pubs, uint8_t* terms) {
+  if (!ctx || !pubs || !terms) return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, 1)) return rc;
+  std::vector<uint8_t> canon(pubs, pubs + 128 * n), fac(32 * n);
+  for (size_t i = 0; i < 4 * n; i++) bn256_reduce32(canon.data() + 32 * i);
+  if (int rc = b2k_bdn_coefficients(n, canon.data(), 128, 1, fac.data())) return rc;
+  return b2k_bn256_g2_mul_batch(ctx, n, fac.data(), canon.data(), terms);
+}
+
+int b2k_bls12381_g2_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, uint8_t* out) {
+  return aggregate_host(ctx, BDN_BLS_G2, n, terms, m, masks, out);
+}
+int b2k_bls12381_g2_bdn_aggregate_keys_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks, void* d_out) {
+  return aggregate_dev(ctx, BDN_BLS_G2, n, d_terms, m, d_masks, d_out);
+}
+int b2k_bls12381_g1_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, uint8_t* out) {
+  return aggregate_host(ctx, BDN_BLS_G1, n, terms, m, masks, out);
+}
+int b2k_bls12381_g1_bdn_aggregate_keys_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks, void* d_out) {
+  return aggregate_dev(ctx, BDN_BLS_G1, n, d_terms, m, d_masks, d_out);
+}
+int b2k_bn256_g2_bdn_aggregate_keys(b2k_ctx* ctx, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, uint8_t* out) {
+  return aggregate_host(ctx, BDN_BN256_G2, n, terms, m, masks, out);
+}
+
+}  // extern "C"

@@ -3,6 +3,7 @@
 #include "msm_host.cuh"
 #include "h2c_g2.cuh"
 #include "pairing_kernels.cuh"
+#include "bdn.cuh"
 using namespace b2k_host;
 
 namespace b2k {
@@ -109,22 +110,21 @@ void verify_layout(Carve& c, VerifyScratch& s, size_t n, bool sig_g1) {
   s.gen = c.take<uint8_t>(pk_bytes);
 }
 
-// ok[i] = bls.Verify(pk_i, msg_i, sig_i), every buffer on the device:
-//   sig_g1: UnmarshalBinary(pk in G2), UnmarshalBinary(sig in G1), H(msg) in G1, e(H(m), pk) == e(sig, G2 generator)
+// bls.Verify's key-independent tail, every buffer on the device: the generator (in the key's group), UnmarshalBinary of the
+// signatures (ok2), H(msg), and the pairing check of s.pk (decoded by the caller, with its flags in ok1) against them:
+//   sig_g1: e(H(m), pk) == e(sig, G2 generator)
 //   else (bls.NewSchemeOnG2, sign/bls/bls.go:48-59): pk in G1, sig in G2, H(msg) in G2, e(pk, H(m)) == e(G1 base, sig)
-int verify_enqueue(b2k_ctx* ctx, bool sig_g1, const VerifyScratch& s, size_t n, const void* pks, const void* msgs, const void* offsets,
-                   const void* dst, uint32_t dst_len, const void* sigs, void* ok) {
+// Shared by bls.Verify (verify_enqueue) and the BDN batch, whose keys are aggregates (bdn_verify_enqueue).
+int verify_tail(b2k_ctx* ctx, bool sig_g1, const VerifyScratch& s, size_t n, const void* msgs, const void* offsets, const void* dst,
+                uint32_t dst_len, const void* sigs, void* ok) {
   cudaStream_t st = ctx->stream;
-  const uint8_t *m = (const uint8_t*)msgs, *d = (const uint8_t*)dst;
+  const uint8_t *m = (const uint8_t*)msgs, *d = (const uint8_t*)dst, *g = (const uint8_t*)sigs;
   const uint32_t* o = (const uint32_t*)offsets;
-  const uint8_t *p = (const uint8_t*)pks, *g = (const uint8_t*)sigs;
   if (sig_g1) {
     k_write_g2_generator<<<1, 32, 0, st>>>(s.gen);
-    k_g2_decompress_v<<<blocks_of(n, 64), 64, 0, st>>>(n, p, s.pk, s.ok1);
     k_g1_decompress_v<<<blocks_of(n, 128), 128, 0, st>>>(n, g, s.sg, s.ok2);
   } else {
     k_write_g1_generator<<<1, 32, 0, st>>>(s.gen);
-    k_g1_decompress_v<<<blocks_of(n, 128), 128, 0, st>>>(n, p, s.pk, s.ok1);
     k_g2_decompress_v<<<blocks_of(n, 64), 64, 0, st>>>(n, g, s.sg, s.ok2);
   }
   k_and_flags<<<blocks_of(n, 256), 256, 0, st>>>(n, s.ok1, s.ok2, s.okc);
@@ -136,8 +136,74 @@ int verify_enqueue(b2k_ctx* ctx, bool sig_g1, const VerifyScratch& s, size_t n, 
     b2k_internal_launch_pairing_check(ctx, n, s.pk, s.hm, s.gen, s.sg, (uint8_t*)ok, 2, s.okc);   // b = (base [shared], sig)
   }
   CK(cudaGetLastError());
-  ctx->launches += 6;
+  ctx->launches += 5;
   return B2K_OK;
+}
+
+// ok[i] = bls.Verify(pk_i, msg_i, sig_i), every buffer on the device: UnmarshalBinary of the keys, then the shared tail
+int verify_enqueue(b2k_ctx* ctx, bool sig_g1, const VerifyScratch& s, size_t n, const void* pks, const void* msgs, const void* offsets,
+                   const void* dst, uint32_t dst_len, const void* sigs, void* ok) {
+  const uint8_t* p = (const uint8_t*)pks;
+  if (sig_g1) k_g2_decompress_v<<<blocks_of(n, 64), 64, 0, ctx->stream>>>(n, p, s.pk, s.ok1);
+  else k_g1_decompress_v<<<blocks_of(n, 128), 128, 0, ctx->stream>>>(n, p, s.pk, s.ok1);
+  CK(cudaGetLastError());
+  ctx->launches += 1;
+  return verify_tail(ctx, sig_g1, s, n, msgs, offsets, dst, dst_len, sigs, ok);
+}
+
+// BDN: bls.Verify under each mask's aggregate key (written straight into the key slots of the tail's scratch), then statuses
+struct BdnVerifyScratch {
+  VerifyScratch v;
+  BdnScratch a;
+  uint8_t* pair_ok;
+};
+void bdn_verify_layout(Carve& c, BdnVerifyScratch& s, size_t n, size_t m, bool sig_g1) {
+  verify_layout(c, s.v, m, sig_g1);
+  bdn_layout(c, s.a, sig_g1 ? BDN_BLS_G2 : BDN_BLS_G1, n, m);
+  s.pair_ok = c.take<uint8_t>(m);
+}
+int bdn_verify_enqueue(b2k_ctx* ctx, bool sig_g1, const BdnVerifyScratch& s, size_t n, const void* terms, size_t m, const void* masks,
+                       const void* msgs, const void* offsets, const void* dst, uint32_t dst_len, const void* sigs, void* status) {
+  int rc = bdn_aggregate_enqueue(ctx, sig_g1 ? BDN_BLS_G2 : BDN_BLS_G1, s.a, n, (const uint8_t*)terms, m, (const uint8_t*)masks,
+                                 s.v.pk, sig_g1 ? 192 : 96);
+  if (rc) return rc;
+  CK(cudaMemsetAsync(s.v.ok1, 1, m, ctx->stream));      // an aggregate key is a point by construction
+  rc = verify_tail(ctx, sig_g1, s.v, m, msgs, offsets, dst, dst_len, sigs, s.pair_ok);
+  if (rc) return rc;
+  return bdn_status_enqueue(ctx, m, s.v.ok2, s.pair_ok, (uint8_t*)status);
+}
+
+int bdn_verify_dev(b2k_ctx* ctx, bool sig_g1, size_t n, const void* d_terms, size_t m, const void* d_masks, const void* d_msgs,
+                   const void* d_offsets, const void* d_dst, uint32_t dst_len, const void* d_sigs, void* d_status) {
+  if (!ctx || !d_terms || !d_masks || !d_msgs || !d_offsets || !d_dst || !d_sigs || !d_status || dst_len == 0 || dst_len > 255)
+    return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, m)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  BdnVerifyScratch s;
+  if (int rc = arena_carve(ctx, [&](Carve& c) { bdn_verify_layout(c, s, n, m, sig_g1); })) return rc;
+  return bdn_verify_enqueue(ctx, sig_g1, s, n, d_terms, m, d_masks, d_msgs, d_offsets, d_dst, dst_len, d_sigs, d_status);
+}
+
+// bad signature data is a status; B2K_ERR_POINT comes only from a malformed term and stays a call error
+int bdn_verify_host(b2k_ctx* ctx, bool sig_g1, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, const uint8_t* msgs,
+                    const uint32_t* offsets, const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs, uint8_t* status) {
+  if (!ctx || !terms || !masks || !msgs || !offsets || !dst || !sigs || !status || dst_len == 0 || dst_len > 255) return B2K_ERR_ARG;
+  if (int rc = bdn_args(ctx, n, m)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  if (check_offsets(ctx, m, offsets)) return B2K_ERR_ARG;
+  BdnVerifyScratch s;
+  uint8_t *d_terms = nullptr, *d_masks = nullptr, *d_sig = nullptr, *d_msg = nullptr, *d_dst = nullptr, *d_status = nullptr;
+  uint32_t* d_off = nullptr;
+  return host_call(ctx, [&](Carve& c) {
+    d_terms = c.in(terms, n, sig_g1 ? 192 : 96);
+    d_masks = c.in(masks, m, (n + 7) / 8);
+    d_sig = c.in(sigs, m, sig_g1 ? 48 : 96);
+    d_msg = c.in(msgs, offsets[m]);
+    d_off = c.in(offsets, m + 1);
+    d_dst = c.in(dst, dst_len);
+    d_status = c.out(status, m);
+    bdn_verify_layout(c, s, n, m, sig_g1);
+  }, [&] { return bdn_verify_enqueue(ctx, sig_g1, s, n, d_terms, m, d_masks, d_msg, d_off, d_dst, dst_len, d_sig, d_status); });
 }
 
 int verify_dev(b2k_ctx* ctx, bool sig_g1, size_t n, const void* d_pks, const void* d_msgs, const void* d_offsets, const void* d_dst,
@@ -224,6 +290,24 @@ int b2k_bls12381_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* pks96, cons
 int b2k_bls12381_verify_g2sig(b2k_ctx* ctx, size_t n, const uint8_t* pks48, const uint8_t* msgs, const uint32_t* offsets,
                               const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs96, uint8_t* ok) {
   return verify_host(ctx, false, n, pks48, msgs, offsets, dst, dst_len, sigs96, ok);
+}
+
+// sign/bdn: bls.Verify under the aggregate key of each mask over one roster's terms (b2k_bdn.cu aggregates)
+int b2k_bls12381_bdn_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, const uint8_t* msgs,
+                                  const uint32_t* offsets, const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs, uint8_t* status) {
+  return bdn_verify_host(ctx, true, n, terms, m, masks, msgs, offsets, dst, dst_len, sigs, status);
+}
+int b2k_bls12381_bdn_verify_g1sig_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks, const void* d_msgs,
+                                      const void* d_offsets, const void* d_dst, uint32_t dst_len, const void* d_sigs, void* d_status) {
+  return bdn_verify_dev(ctx, true, n, d_terms, m, d_masks, d_msgs, d_offsets, d_dst, dst_len, d_sigs, d_status);
+}
+int b2k_bls12381_bdn_verify_g2sig(b2k_ctx* ctx, size_t n, const uint8_t* terms, size_t m, const uint8_t* masks, const uint8_t* msgs,
+                                  const uint32_t* offsets, const uint8_t* dst, uint32_t dst_len, const uint8_t* sigs, uint8_t* status) {
+  return bdn_verify_host(ctx, false, n, terms, m, masks, msgs, offsets, dst, dst_len, sigs, status);
+}
+int b2k_bls12381_bdn_verify_g2sig_dev(b2k_ctx* ctx, size_t n, const void* d_terms, size_t m, const void* d_masks, const void* d_msgs,
+                                      const void* d_offsets, const void* d_dst, uint32_t dst_len, const void* d_sigs, void* d_status) {
+  return bdn_verify_dev(ctx, false, n, d_terms, m, d_masks, d_msgs, d_offsets, d_dst, dst_len, d_sigs, d_status);
 }
 
 }  // extern "C"

@@ -20,6 +20,8 @@ WATCH = {  # kernel name fragment -> max instructions of its largest 12-limb pro
     "k_msm_accumulate_slicesINS_8Bls381G2": 420, "k_msm_reduce_l1INS_8Bls381G2": 420, "k_msm_accumulateINS_8Bls381G2": 420,   # b2k_g2.o
     "k_msm_accumulate_slices_directINS_8Bls381G1": 420, "k_pt_backwardINS_8Bls381G1": 420,                                  # b2k_api.o
     "k_msm_accumulate_slicesINS_8Bls381G1ELi3": 420,                                 # the slice kernel the automatic plan runs
+    "k_bdn_masked_sumINS_8Bls381G2": 420, "k_bdn_masked_sumINS_8Bls381G1": 420,      # sign/bdn's masked sums (b2k_bdn.o)
+    "k_bdn_finishINS_8Bls381G2": 420, "k_bdn_totalINS_8Bls381G2": 420,
 }
 
 
