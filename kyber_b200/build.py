@@ -47,9 +47,8 @@ def _closure(src: str) -> list:
     return [seen[0]] + sorted(seen[1:])
 
 
-def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile kyber_b200/libb2kyber.so.  Incremental per translation unit: a unit is recompiled when its own source or a
-    header it includes (transitively) changed (stamp next to the object), the library is relinked when an object changed.  Returns the library path."""
+def generate_tables() -> None:
+    """Write the generated tables the device headers include, when missing or older than their generator."""
     # the program tables of the warp-cooperative pairing are generated (1 s, pure Python, the curve's public parameters only): tools/gen_coop_pairing.py
     gen = os.path.join(HERE, "..", "tools", "gen_coop_pairing.py")
     incs = [os.path.join(CSRC, f"coop_program_{c}.inc") for c in ("bls", "bn254", "bn256")]
@@ -60,6 +59,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
     inc = os.path.join(CSRC, "ecies_base_comb.inc")
     if not os.path.exists(inc) or os.path.getmtime(inc) < os.path.getmtime(gen_ecies):
         subprocess.run([sys.executable, gen_ecies], check=True, stdout=subprocess.DEVNULL)
+
+
+def build(force: bool = False, verbose: bool = False) -> str:
+    """Compile kyber_b200/libb2kyber.so.  Incremental per translation unit: a unit is recompiled when its own source or a
+    header it includes (transitively) changed (stamp next to the object), the library is relinked when an object changed.  Returns the library path."""
+    generate_tables()
     objs, procs = [], []
     for u in UNITS:
         src = os.path.join(CSRC, u)

@@ -19,21 +19,6 @@ void emul_counts(uint64_t* out, int reset) {
   if (reset) memset(ecies_counts, 0, sizeof(ecies_counts));
 }
 
-// one AES-256 block (the second lane of the two-block call carries a zero block)
-void emul_aes256(const uint8_t* key, const uint8_t* in, uint8_t* out) {
-  uint8_t rk[240], b[32] = {};
-  aes256_expand(rk, key);
-  memcpy(b, in, 16);
-  aes256_encrypt2(b, rk);
-  memcpy(out, b, 16);
-}
-
-void emul_kdf(const uint8_t* dh, uint8_t* out44) { ecies_kdf(out44, dh); }
-
-void emul_gcm_seal(const uint8_t* k44, const uint8_t* msg, uint32_t len, uint8_t* out) { gcm_seal(k44, msg, len, out); }
-
-int emul_gcm_open(const uint8_t* k44, const uint8_t* ct, uint32_t clen, uint8_t* msg) { return gcm_open(k44, ct, clen, msg) ? 1 : 0; }
-
 // geScalarMult(s, P) through the constant-time table and selection; -1 if P does not decode
 int emul_mul_var(const uint8_t* s, const uint8_t* p, uint8_t* out) {
   EdExt P, Q;

@@ -39,13 +39,6 @@ int emul_ed_load(const uint8_t* scalar, const uint8_t* point, int c, int16_t* di
   return ok ? 1 : 0;
 }
 
-void emul_ed_scalar_rule(const uint8_t* k_in, uint8_t* k_out) {
-  uint32_t k[8];
-  sc_load_le(k, k_in);
-  ed_scalar_rule(k);
-  for (int j = 0; j < 32; j++) k_out[j] = (uint8_t)(k[j >> 2] >> (8 * (j & 3)));
-}
-
 // The whole MSM with window c, chunk m, slice length L; buckets with more than serial_max partials (2 or 64) take the
 // block-parallel fix-up.  Returns the number of points that did not decode; stats = {cut buckets, block-parallel buckets}.
 int emul_ed_msm(uint32_t n, const uint8_t* scalars, const uint8_t* points, int c, int m, uint32_t L, int serial_max, uint8_t* out,

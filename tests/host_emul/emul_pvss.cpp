@@ -9,43 +9,6 @@ static void limbs_to_le(uint8_t* out, const uint32_t* s) {
 }
 
 extern "C" {
-// BLAKE2b-512 of msg with the given parameter words 0..2 (RFC 7693 with an explicit parameter block; no key)
-void emul_blake2b(const uint8_t* msg, uint32_t len, uint64_t p0, uint64_t p1, uint64_t p2, uint8_t* out) {
-  uint64_t h[8];
-  blake2b_init(h, p0, p1, p2);
-  const uint32_t nblk = len ? (len + 127) / 128 : 1;
-  for (uint32_t b = 0; b < nblk; b++) {
-    uint64_t m[16];
-    for (int i = 0; i < 16; i++) {
-      uint64_t w = 0;
-      for (int j = 7; j >= 0; j--) {
-        const uint32_t pos = 128 * b + 8 * i + j;
-        w = (w << 8) | (pos < len ? msg[pos] : 0);
-      }
-      m[i] = w;
-    }
-    blake2b_compress(h, m, 128 * (b + 1) < len ? 128 * (b + 1) : len, b == nblk - 1);
-  }
-  for (int i = 0; i < 64; i++) out[i] = (uint8_t)(h[i >> 3] >> (8 * (i & 7)));
-}
-
-// the root hash and output blocks 0..nblk-1 of blake2xb.New(seed)
-void emul_blake2xb(const uint8_t* seed, uint32_t len, uint32_t nblk, uint8_t* root, uint8_t* out) {
-  uint64_t h0[8], b[8];
-  blake2xb_root(h0, seed, len);
-  for (int i = 0; i < 64; i++) root[i] = (uint8_t)(h0[i >> 3] >> (8 * (i & 7)));
-  for (uint32_t k = 0; k < nblk; k++) {
-    blake2xb_block(b, h0, k);
-    for (int i = 0; i < 64; i++) out[64 * k + i] = (uint8_t)(b[i >> 3] >> (8 * (i & 7)));
-  }
-}
-
-void emul_sc_pick(const uint8_t* seed, uint32_t len, uint8_t* out) {
-  uint32_t s[8];
-  sc_pick(s, seed, len);
-  limbs_to_le(out, s);
-}
-
 // geScalarMult(r, P) + geScalarMult(c, P2), encoded; false if a point does not decode
 int emul_double_mul_var(const uint8_t* r, const uint8_t* p, const uint8_t* c, const uint8_t* p2, uint8_t* out) {
   EdExt P, P2, Q;

@@ -53,13 +53,6 @@ int emul_phi_term(const uint8_t* zs, const uint8_t* p, const uint8_t* zr, const 
   return 1;
 }
 
-void emul_neg_mod_l(const uint8_t* b, uint8_t* out) {
-  uint32_t s[8], r[8];
-  sc_load_le(s, b);
-  sc_neg_mod_l(r, s);
-  for (int j = 0; j < 32; j++) out[j] = (uint8_t)(r[j >> 2] >> (8 * (j & 3)));
-}
-
 // GetSequenceVerifiable of one output point over nq rows pts[nq][32], e[nq][32]; 0 if a point does not decode
 int emul_sequence_term(uint32_t nq, const uint8_t* pts, const uint8_t* e, uint8_t* out) {
   std::vector<EdAff> a(nq);

@@ -1,7 +1,8 @@
 """CPU: ECIES's device bodies (kyber_b200/csrc/ecies.cuh) compiled for the host and checked against the restatement in
-oracle/ecies.py -- the AES-256 block, GCM Seal and Open across block edges, HKDF, both constant-time multiplications against
-point_mul (top-bit scalars, the identity, small-order points, all-zero bytes), whole encryptions and decryptions, and the
-operation counts of the constant-time helpers, which must not depend on the key, r, the point or the message."""
+oracle/ecies.py -- both constant-time multiplications against point_mul (top-bit scalars, the identity, small-order points,
+all-zero bytes), whole encryptions and decryptions, and the operation counts of the constant-time helpers, which must not depend
+on the key, r, the point or the message.  AES-256, GHASH, GCM Seal and Open and HKDF are checked on their own by the byte
+harness (test_bytes_emulation.py, test_gpu_bytes.py)."""
 import ctypes
 import os
 import random
@@ -16,7 +17,6 @@ from oracle import ed25519 as ed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "host_emul", "emul_ecies.cpp")
-LENGTHS = [0, 1, 15, 16, 17, 31, 32, 33, 4096]
 IDENT = ed.encode(ed.IDENT)
 T8 = mc.T8                                                  # a point of order 8
 
@@ -33,10 +33,6 @@ def lib(tmp_path_factory):
     lib = ctypes.CDLL(so)
     u32, sz, cp = ctypes.c_uint32, ctypes.c_size_t, ctypes.c_char_p
     lib.emul_counts.argtypes = [ctypes.c_void_p, ctypes.c_int]
-    lib.emul_aes256.argtypes = [cp] * 3
-    lib.emul_kdf.argtypes = [cp, cp]
-    lib.emul_gcm_seal.argtypes = [cp, cp, u32, cp]
-    lib.emul_gcm_open.argtypes = [cp, cp, u32, cp]
     lib.emul_mul_var.argtypes = [cp] * 3
     lib.emul_mul_base.argtypes = [cp] * 2
     lib.emul_decrypt.argtypes = [cp, sz, u32, cp, cp, cp]
@@ -64,42 +60,6 @@ def encrypt(lib, pubs, rs, msgs):
     lib.emul_encrypt(n, b"".join(pubs), b"".join(rs), ln, b"".join(msgs) or b"\x00", out, st)
     w = ln + 48
     return [(st.raw[i], out.raw[w * i:w * i + w]) for i in range(n)]
-
-
-def test_aes256_block(lib):
-    out = ctypes.create_string_buffer(16)
-    lib.emul_aes256(bytes(range(32)), bytes.fromhex("00112233445566778899aabbccddeeff"), out)
-    assert out.raw == bytes.fromhex("8ea2b7ca516745bfeafc49904b496089")
-    rng = random.Random(1)
-    for _ in range(20):
-        key, blk = rng.randbytes(32), rng.randbytes(16)
-        lib.emul_aes256(key, blk, out)
-        assert out.raw == ec.aes256_encrypt_block(key, blk)
-
-
-def test_hkdf(lib):
-    rng = random.Random(2)
-    out = ctypes.create_string_buffer(44)
-    for dh in [bytes(32), b"\xff" * 32] + [rng.randbytes(32) for _ in range(10)]:
-        lib.emul_kdf(dh, out)
-        assert out.raw == ec.hkdf_sha256(dh, 44)
-
-
-@pytest.mark.parametrize("n", LENGTHS)
-def test_gcm_seal_and_open(lib, n):
-    rng = random.Random(100 + n)
-    k44, msg = rng.randbytes(44), rng.randbytes(n)
-    out = ctypes.create_string_buffer(n + 16)
-    lib.emul_gcm_seal(k44, msg, n, out)
-    assert out.raw == ec.gcm_seal(k44[:32], k44[32:], msg)
-    back = ctypes.create_string_buffer(max(n, 1))
-    assert lib.emul_gcm_open(k44, out.raw, n + 16, back) == 1 and back.raw[:n] == msg
-    for pos in {0, n // 2, n + 15}:
-        bad = bytearray(out.raw)
-        bad[pos] ^= 0x01
-        back = ctypes.create_string_buffer(b"\xaa" * max(n, 1))
-        assert lib.emul_gcm_open(k44, bytes(bad), n + 16, back) == 0
-        assert back.raw[:n] == bytes(n)
 
 
 def scalars(rng):

@@ -25,7 +25,6 @@ def lib(tmp_path_factory):
                    check=True)
     lib = ctypes.CDLL(so)
     lib.emul_ed_load.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_char_p]
-    lib.emul_ed_scalar_rule.argtypes = [ctypes.c_char_p, ctypes.c_char_p]
     lib.emul_ed_msm.argtypes = [ctypes.c_uint32, ctypes.c_char_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_int, ctypes.c_uint32,
                                 ctypes.c_int, ctypes.c_char_p, ctypes.c_void_p]
     lib.emul_ed_lagrange.argtypes = [ctypes.c_uint32, ctypes.c_char_p, ctypes.c_char_p]
@@ -42,15 +41,6 @@ def _msm(lib, scalars, pts: bytes, c, m, L, serial_max=64):
     out, stats = ctypes.create_string_buffer(32), (ctypes.c_uint32 * 2)()
     bad = lib.emul_ed_msm(len(scalars), cases.le(scalars), pts, c, m, L, serial_max, out, stats)
     return out.raw, bad, (stats[0], stats[1])
-
-
-def test_scalar_rule_matches_the_oracle(lib):
-    rng = random.Random(1)
-    ks = cases.crafted_high_scalars(rng) + [rng.getrandbits(256) for _ in range(3000)] + [0, 1, ed.L, (1 << 255) - 1]
-    for k in ks:
-        out = ctypes.create_string_buffer(32)
-        lib.emul_ed_scalar_rule(k.to_bytes(32, "little"), out)
-        assert int.from_bytes(out.raw, "little") == cases.effective_scalar(k), hex(k)
 
 
 @pytest.mark.parametrize("c", WINDOWS)

@@ -1,9 +1,8 @@
-"""CPU: the Ed25519 verification device code (kyber_b200/csrc/eddsa.cuh) compiled for the host and checked against
-hashlib, Python integers and the oracle on every fixture and crafted case -- the same bodies k_ed25519_verify runs."""
+"""CPU: the Ed25519 verification device code (kyber_b200/csrc/eddsa.cuh) compiled for the host and checked against the oracle
+on every fixture and crafted case -- the same bodies k_ed25519_verify runs.  SHA-512 and the reduction mod l are checked on
+their own by the byte harness (test_bytes_emulation.py, test_gpu_bytes.py)."""
 import ctypes
-import hashlib
 import os
-import random
 import subprocess
 
 import pytest
@@ -22,35 +21,8 @@ def lib(tmp_path_factory):
     subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-std=c++17", "-DB2K_HOST_EMUL", "-Wno-unknown-pragmas", SRC, "-o", so],
                    check=True)
     lib = ctypes.CDLL(so)
-    lib.emul_sha512_3.argtypes = [ctypes.c_char_p, ctypes.c_uint32] * 3 + [ctypes.c_char_p]
     lib.emul_ed25519_verify.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_uint32, ctypes.c_char_p]
     return lib
-
-
-def _sha(lib, a=b"", b=b"", c=b""):
-    out = ctypes.create_string_buffer(64)
-    lib.emul_sha512_3(a, len(a), b, len(b), c, len(c), out)
-    return out.raw
-
-
-def test_sha512_matches_hashlib_on_every_length(lib):
-    rng = random.Random(5)
-    for n in list(range(0, 301)) + [1023, 100000]:
-        d = bytes(rng.getrandbits(8) for _ in range(n))
-        want = hashlib.sha512(d).digest()
-        assert _sha(lib, c=d) == want, n
-        if n >= 64:                                      # the verifier's split: R || A || M
-            assert _sha(lib, d[:32], d[32:64], d[64:]) == want, n
-
-
-def test_reduce512_matches_python(lib):
-    L = ed.L
-    rng = random.Random(7)
-    vals = [0, L - 1, L, L + 1, 2 * L, 3 * L - 1, 2 ** 512 - 1, 2 ** 256, 2 ** 253 - 1] + [rng.getrandbits(512) for _ in range(2000)]
-    for v in vals:
-        out = ctypes.create_string_buffer(32)
-        lib.emul_reduce512(v.to_bytes(64, "little"), out)
-        assert int.from_bytes(out.raw, "little") == v % L, hex(v)
 
 
 def test_generated_base_table_matches_the_oracle(lib):

@@ -1,8 +1,8 @@
-"""CPU: the DLEQ / PVSS device code (kyber_b200/csrc/pvss.cuh) compiled for the host and checked against hashlib and the
-restatement in tests/pvss_cases.py -- BLAKE2b, the keyed XOF, sc_pick across rejections, the joint multiplication over two
-variable bases on both sides of the top-digit rule, the per-share and per-deal challenges."""
+"""CPU: the DLEQ / PVSS device code (kyber_b200/csrc/pvss.cuh) compiled for the host and checked against the restatement in
+tests/pvss_cases.py -- the joint multiplication over two variable bases on both sides of the top-digit rule, the per-share and
+per-deal challenges.  BLAKE2b, the keyed XOF and sc_pick are checked on their own by the byte harness (test_bytes_emulation.py,
+test_gpu_bytes.py)."""
 import ctypes
-import hashlib
 import os
 import random
 import subprocess
@@ -23,58 +23,12 @@ def lib(tmp_path_factory):
     subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-std=c++17", "-DB2K_HOST_EMUL", "-Wno-unknown-pragmas", SRC, "-o", so],
                    check=True)
     lib = ctypes.CDLL(so)
-    u32, u64, cp = ctypes.c_uint32, ctypes.c_uint64, ctypes.c_char_p
-    lib.emul_blake2b.argtypes = [cp, u32, u64, u64, u64, cp]
-    lib.emul_blake2xb.argtypes = [cp, u32, u32, cp, cp]
-    lib.emul_sc_pick.argtypes = [cp, u32, cp]
+    u32, cp = ctypes.c_uint32, ctypes.c_char_p
     lib.emul_double_mul_var.argtypes = [cp] * 5
     lib.emul_dleq_verify.argtypes = [cp] * 5
     lib.emul_dec_share.argtypes = [cp] * 5
     lib.emul_enc_shares.argtypes = [u32, u32] + [cp] * 8
     return lib
-
-
-def test_blake2b_matches_hashlib(lib):
-    rng = random.Random(1)
-    for n in list(range(0, 260)) + [1000, 4096]:
-        d = bytes(rng.getrandbits(8) for _ in range(n))
-        out = ctypes.create_string_buffer(64)
-        lib.emul_blake2b(d, n, 0x01010040, 0, 0, out)
-        assert out.raw == hashlib.blake2b(d).digest(), n
-
-
-@pytest.mark.parametrize("klen", list(range(0, 65)) + [65, 96, 127, 128, 129, 200, 300])
-def test_keyed_xof_matches_the_restatement_and_hashlib(lib, klen):
-    rng = random.Random(100 + klen)
-    seed = bytes(rng.getrandbits(8) for _ in range(klen))
-    root, out = ctypes.create_string_buffer(64), ctypes.create_string_buffer(64 * 3)
-    lib.emul_blake2xb(seed, klen, 3, root, out)
-    x = pc.Xof(seed)
-    assert root.raw == x.root == hashlib.blake2b(seed[64:], digest_size=64, key=seed[:64], fanout=1, depth=1,
-                                                 node_offset=0xFFFFFFFF << 32).digest()
-    assert out.raw == x.read(64 * 3)
-
-
-def _pick(lib, seed):
-    out = ctypes.create_string_buffer(32)
-    lib.emul_sc_pick(seed, len(seed), out)
-    return out.raw
-
-
-def test_sc_pick_across_rejections(lib):
-    found = {}
-    for i in range(4000):
-        seed = hashlib.sha256(b"pick %d" % i).digest()
-        k = pc.pick_draws(seed)
-        if k not in found:
-            found[k] = seed
-        if all(j in found for j in (1, 2, 3, 4)):
-            break
-    assert all(j in found for j in (1, 2, 3, 4)), sorted(found)       # first one, two, three draws rejected
-    for seed in found.values():
-        assert _pick(lib, seed) == pc.pick(pc.Xof(seed))
-    for seed in (b"", b"example", bytes(64), bytes(100)):
-        assert _pick(lib, seed) == pc.pick(pc.Xof(seed))
 
 
 def test_double_mul_var_is_the_sum_of_two_reference_multiplications(lib):

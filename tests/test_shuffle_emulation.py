@@ -1,6 +1,6 @@
 """CPU: the shuffle verifier's device bodies (kyber_b200/csrc/shuffle.cuh) and host transcript (shuffle_transcript.h) compiled
 for the host and checked against the restatement in tests/shuffle_cases.py -- thver with raw and e63-rule scalars, the Phi term
-and the single multiplication on torsion points, (-b) mod l, the sequence term, the threaded Pick squeeze, the transcript, and
+and the single multiplication on torsion points, the sequence term, the threaded Pick squeeze, the transcript, and
 whole batches through every kernel body in order."""
 import ctypes
 import os
@@ -30,7 +30,6 @@ def lib(tmp_path_factory):
     lib.emul_pick_many.restype = ctypes.c_uint64
     lib.emul_thver.argtypes = [cp] * 5
     lib.emul_phi_term.argtypes = [cp] * 6
-    lib.emul_neg_mod_l.argtypes = [cp, cp]
     lib.emul_sequence_term.argtypes = [u32, cp, cp, cp]
     lib.emul_shuffle_verify.argtypes = [sz, sz] + [cp] * 7 + [cp, u32, cp]
     return lib
@@ -39,14 +38,6 @@ def lib(tmp_path_factory):
 def scalars(rng):
     return mc.crafted_high_scalars(rng) + [0, 1, L - 1, L, L + 1, (1 << 255) - 1, (1 << 256) - 1] + \
         [rng.getrandbits(256) for _ in range(4)]
-
-
-def test_neg_mod_l(lib):
-    rng = random.Random(1)
-    for b in scalars(rng):
-        out = ctypes.create_string_buffer(32)
-        lib.emul_neg_mod_l(sc.le(b), out)
-        assert int.from_bytes(out.raw, "little") == (-b) % L, hex(b)
 
 
 def test_thver_raw_a_and_negated_b(lib):
