@@ -752,6 +752,37 @@ int b2k_bn256_bdn_verify_g1sig(b2k_ctx* ctx, size_t n, const uint8_t* terms /*[n
                                const uint8_t* masks /*[m][(n+7)/8]*/, const uint8_t* msgs, const uint32_t* offsets /*[m+1]*/,
                                const uint8_t* sigs /*[m][64]*/, uint8_t* status /*[m]*/);
 
+/* ---- sign/schnorr over BLS12-381 keys on G1 or on G2 ------------------------------------------------------------------------
+ * status[i] = 0 iff schnorr.VerifyWithChecks(suite.G1() or suite.G2(), pks[i], msg_i, sigs[i]) == nil
+ * (sign/schnorr/schnorr.go:89-183), else the code of the FIRST check that fails, in the reference's order:
+ *   1 B2K_SCHNORR_R        R (the first 48 / 96 bytes of sig) does not decode: kilic's UnmarshalBinary error (ZCash flags,
+ *                          x < p, on the curve, in the order-r subgroup: b2k_bls12381_g{1,2}_decompress)
+ *   2 B2K_SCHNORR_S        s (the last 32 bytes, big-endian) >= r: mod.Int's "UnmarshalBinary: value out of range"
+ *   3 B2K_SCHNORR_PK       the key does not decode: "schnorr: error unmarshalling public key"
+ *   4 B2K_SCHNORR_INVALID  s B != R + h public, h = SHA-512(R || public || msg) read big-endian mod r: "schnorr: invalid signature"
+ * The reference's "point not in correct group" (R.IsInCorrectGroup) cannot fail on this backend: UnmarshalBinary already
+ * refused every point outside the subgroup.  Neither kilic's points nor mod.Int have IsCanonical / HasSmallOrder, so those
+ * checks do not apply.  The digest hashes the input bytes of R and of the key: the decoders accept only encodings that are
+ * their own MarshalBinary.  Infinity is a valid R and a valid key, as in the reference: with the key at infinity a signature
+ * is valid iff s B = R, and (R, s, key) = (O, 0, O) is accepted.
+ * Signatures (R || s: 80 bytes with keys on G1, 128 on G2) and keys have a fixed stride, so the reference's length error is
+ * the caller's check.  msgs/offsets as in b2k_ed25519_verify.  Bad data is never a call error, only a status; n == 0, a null
+ * pointer or decreasing offsets (host forms) -> B2K_ERR_ARG.  The host forms stage every input in one device allocation and
+ * synchronise; the _dev forms take device pointers and only enqueue.
+ * replaces: schnorr.Verify / VerifyWithChecks called once per packet, e.g. dkg.VerifyPacketSignature
+ * (share/dkg/pedersen/structs.go:293-348, protocol.go:275-281), share/vss/pedersen vss.go:439, 675, share/vss/rabin
+ * vss.go:485, 677, share/dkg/rabin dkg.go:454, 494, 563.  On edwards25519, b2k_ed25519_verify is the device path: the two
+ * schemes accept exactly the same signatures there. */
+enum { B2K_SCHNORR_OK = 0, B2K_SCHNORR_R = 1, B2K_SCHNORR_S = 2, B2K_SCHNORR_PK = 3, B2K_SCHNORR_INVALID = 4 };
+int b2k_bls12381_g1_schnorr_verify(b2k_ctx* ctx, size_t n, const uint8_t* pks /*[n][48]*/, const uint8_t* msgs,
+                                   const uint32_t* offsets /*[n+1]*/, const uint8_t* sigs /*[n][80] R||s*/, uint8_t* status /*[n]*/);
+int b2k_bls12381_g1_schnorr_verify_dev(b2k_ctx* ctx, size_t n, const void* d_pks, const void* d_msgs, const void* d_offsets,
+                                       const void* d_sigs, void* d_status);
+int b2k_bls12381_g2_schnorr_verify(b2k_ctx* ctx, size_t n, const uint8_t* pks /*[n][96]*/, const uint8_t* msgs,
+                                   const uint32_t* offsets /*[n+1]*/, const uint8_t* sigs /*[n][128] R||s*/, uint8_t* status /*[n]*/);
+int b2k_bls12381_g2_schnorr_verify_dev(b2k_ctx* ctx, size_t n, const void* d_pks, const void* d_msgs, const void* d_offsets,
+                                       const void* d_sigs, void* d_status);
+
 #ifdef __cplusplus
 }
 #endif

@@ -539,6 +539,24 @@ class Engine:
         """the same on device pointers ([n][32], message bytes, [n+1] uint32 offsets, [n][64], [n] status); enqueue only"""
         self._call("b2k_ed25519_verify_dev", n, d_pks, d_msgs, d_offsets, d_sigs, d_status)
 
+    SCHNORR_POINT_BYTES = {"bls12381_g1": 48, "bls12381_g2": 96}
+
+    def schnorr_verify(self, group: str, pks: bytes, msgs, sigs: bytes) -> bytes:
+        """n x schnorr.VerifyWithChecks over BLS12-381 keys on G1 or G2 (group "bls12381_g1" / "bls12381_g2"): pks [n][48 or 96],
+        msgs list of bytes, sigs [n][80 or 128] R || s -> one status byte each (B2K_SCHNORR_* of include/b2kyber.h)"""
+        pl = self.SCHNORR_POINT_BYTES[group]
+        n = len(msgs)
+        assert len(pks) == pl * n and len(sigs) == (pl + 32) * n
+        blob, offs = self._pack_msgs(msgs)
+        return self._call(f"b2k_{group}_schnorr_verify", n, pks, blob, offs, sigs, out=n)
+
+    def schnorr_verify_dev(self, group: str, n: int, d_pks: int, d_msgs: int, d_offsets: int, d_sigs: int, d_status: int):
+        """the same on device pointers ([n][48 or 96], message bytes, [n+1] uint32 offsets, [n][80 or 128], [n] status);
+        enqueue only"""
+        if group not in self.SCHNORR_POINT_BYTES:
+            raise ValueError(f"unknown group {group!r}")
+        self._call(f"b2k_{group}_schnorr_verify_dev", n, d_pks, d_msgs, d_offsets, d_sigs, d_status)
+
     def ed25519_dleq_verify(self, g: bytes, h: bytes, xg: bytes, xh: bytes, proofs: bytes) -> bytes:
         """n x dleq.Proof.Verify(G, H, xG, xH): points [n][32], proofs [n][128] C || R || VG || VH -> one status byte each
         (B2K_DLEQ_*: 0 OK, 2 INVALID, 3 POINT)"""
