@@ -640,6 +640,41 @@ int b2k_ed25519_ecies_encrypt(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][
                               size_t len, const uint8_t* msg /*[n][len]*/, uint8_t* ctxt /*[n][32 + len + 16]*/,
                               uint8_t* status /*[n]*/);
 
+/* ---- BLS12-381 ECIES, keys on G1 or on G2 (encrypt/ecies, hash SHA-256) ---------------------------------------------------
+ * Byte for byte ecies.Encrypt / ecies.Decrypt (encrypt/ecies/ecies.go:23-131) with the suite's G1 or G2 as the group and
+ * sha256.New: the Pedersen DKG's Deals (share/dkg/pedersen/dkg.go:377) and ProcessDeals (:478) when its key group is BLS12-381
+ * (keys on G1, or on G2).  A ciphertext is R.MarshalBinary() (48 bytes on G1, 96 on G2, ZCash compressed, kilic/g1.go:119-124,
+ * g2.go:118-123) || AES-256-GCM(body) || tag (16); the AES key and the GCM nonce are HKDF-SHA256(dh.MarshalBinary(), salt nil,
+ * info nil)[0:32] and [32:44] (an ikm of 48 or 96 bytes); no AAD.  R and the public keys decode as UnmarshalBinary does
+ * (compressed form, x < p, on the curve, in the subgroup; infinity only as 0xC0 || 0...).  Scalars (priv, r) are mod.Int bytes:
+ * 32 bytes big-endian; 0 is valid (dh and R are then infinity).  A scalar >= r fails the whole call with B2K_ERR_SCALAR_RANGE
+ * before anything is staged; that check runs on the host as a borrow chain over all 32 bytes of every scalar, without an early
+ * exit.  Bad data is only a status, never a call error.  B2K_ERR_ARG: a null pointer, n == 0, len out of range, or n len too
+ * large.  Blocking, host buffers, staged through the context's input arena, which is cleared before the call returns.
+ *   B2K_ECIES_POINT  R (decrypt) or the public key (encrypt) does not decode (UnmarshalBinary's error); ctxt/msg zeroed
+ *   B2K_ECIES_AUTH   the GCM tag does not match: "cipher: message authentication failed"; msg zeroed
+ * Constant time on the secrets (key, r, dh, R before it is returned, the derived key, AES and GHASH state, plaintext): no
+ * data-dependent branch or address on the device.
+ *   - scalar multiplication: 65 signed radix-16 digits, every digit reads all 8 table entries 1..8 P and keeps one with masks,
+ *     then one complete addition (Renes-Costello-Batina, projective, no case for the identity or P = +-Q), 4 doublings between
+ *     digits; no endomorphism split.  r G runs the same walk over 1..8 G.
+ *   - compression of dh and R: Fermat inversion (on G2 of the norm), sign flag and infinity encoding chosen by masks.
+ *   - AES without tables, GHASH with masks, the tag compared over all 16 bytes (as for edwards25519).
+ * A reference ciphertext shorter than the point length is "invalid ecies cipher"; one too short for a tag fails GCM Open.
+ *   replaces: ecies.Decrypt / ecies.Encrypt called once per ciphertext */
+/* len = ciphertext body incl. tag, 16 <= len <= B2K_ECIES_MAX_LEN + 16; msg[i] zeroed unless OK */
+int b2k_bls12381_g1_ecies_decrypt(b2k_ctx* ctx, const uint8_t* priv /*[32] BE*/, size_t n, size_t len,
+                                  const uint8_t* ctxt /*[n][48 + len]*/, uint8_t* msg /*[n][len - 16]*/, uint8_t* status /*[n]*/);
+int b2k_bls12381_g2_ecies_decrypt(b2k_ctx* ctx, const uint8_t* priv /*[32] BE*/, size_t n, size_t len,
+                                  const uint8_t* ctxt /*[n][96 + len]*/, uint8_t* msg /*[n][len - 16]*/, uint8_t* status /*[n]*/);
+/* len = plaintext length, 0 <= len <= B2K_ECIES_MAX_LEN; ctxt[i] zeroed unless OK */
+int b2k_bls12381_g1_ecies_encrypt(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][48]*/, const uint8_t* r /*[n][32] BE*/,
+                                  size_t len, const uint8_t* msg /*[n][len]*/, uint8_t* ctxt /*[n][48 + len + 16]*/,
+                                  uint8_t* status /*[n]*/);
+int b2k_bls12381_g2_ecies_encrypt(b2k_ctx* ctx, size_t n, const uint8_t* pubs /*[n][96]*/, const uint8_t* r /*[n][32] BE*/,
+                                  size_t len, const uint8_t* msg /*[n][len]*/, uint8_t* ctxt /*[n][96 + len + 16]*/,
+                                  uint8_t* status /*[n]*/);
+
 /* status[i] = 0 iff eddsa.VerifyWithChecks(pks[i], msg_i, sigs[i]) == nil (sign/eddsa/eddsa.go:149-229), else the code of
  * the FIRST check that fails, in the reference's order:
  *   1 s >= l (scalar.IsCanonical)              -> ErrSignatureNotCanonical

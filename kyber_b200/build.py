@@ -9,7 +9,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
               "-Xfatbin", "-compress-all",   # the library is ~85 MB of SASS + line tables uncompressed, ~26 MB compressed
               "-DB2K_COMPACT_FIELD=1"]     # field products as out-of-line by-value calls (fp.cuh); *_inlined.cu units undo it for A/B
-UNITS = ["b2k_api.cu", "b2k_msm_inlined.cu", "b2k_g1_mul.cu", "b2k_bn254.cu", "b2k_g2.cu", "b2k_pairing.cu", "b2k_pairing_inlined.cu", "b2k_h2c.cu", "b2k_share.cu", "b2k_share2.cu", "b2k_ed25519.cu", "b2k_eddsa.cu", "b2k_ed25519_msm.cu", "b2k_pvss.cu", "b2k_shuffle.cu", "b2k_anon.cu", "b2k_bn256.cu", "b2k_bn254_pairing.cu", "b2k_bdn.cu", "b2k_bn_hash.cu", "b2k_bn_codec.cu", "b2k_multi.cu", "b2k_gt.cu", "b2k_ibe.cu", "b2k_ecies.cu", "b2k_schnorr.cu"]
+UNITS = ["b2k_api.cu", "b2k_msm_inlined.cu", "b2k_g1_mul.cu", "b2k_bn254.cu", "b2k_g2.cu", "b2k_pairing.cu", "b2k_pairing_inlined.cu", "b2k_h2c.cu", "b2k_share.cu", "b2k_share2.cu", "b2k_ed25519.cu", "b2k_eddsa.cu", "b2k_ed25519_msm.cu", "b2k_pvss.cu", "b2k_shuffle.cu", "b2k_anon.cu", "b2k_bn256.cu", "b2k_bn254_pairing.cu", "b2k_bdn.cu", "b2k_bn_hash.cu", "b2k_bn_codec.cu", "b2k_multi.cu", "b2k_gt.cu", "b2k_ibe.cu", "b2k_ecies.cu", "b2k_schnorr.cu", "b2k_ecies_bls.cu"]
 
 
 def _nvcc() -> str:

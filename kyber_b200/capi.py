@@ -647,6 +647,31 @@ class Engine:
         w = length + 48
         return [bytes(out[w * i:w * i + w]) for i in range(n)], bytes(status)
 
+    def bls12381_ecies_decrypt(self, group: int, priv: bytes, ctxts, length: int):
+        """n x ecies.Decrypt(BLS12-381 G1 or G2, priv, ctxts[i], sha256.New), group 1 or 2; priv 32 bytes big-endian below r;
+        every ciphertext is 48 (G1) or 96 (G2) + length bytes (length = body + tag, >= 16) -> ([n] messages of length - 16
+        bytes, zero unless OK; n status bytes (B2K_ECIES_*: 0 OK, 1 POINT, 2 AUTH))"""
+        pl = self.POINT_BYTES[f"bls12381_g{group}"][1]
+        n = len(ctxts)
+        assert len(priv) == 32 and all(len(c) == pl + length for c in ctxts)
+        msg, status = bytearray(max(n * (length - 16), 1)), bytearray(n)
+        self._call(f"b2k_bls12381_g{group}_ecies_decrypt", bytes(priv), n, length, b"".join(ctxts), msg, status)
+        w = length - 16
+        return [bytes(msg[w * i:w * i + w]) for i in range(n)], bytes(status)
+
+    def bls12381_ecies_encrypt(self, group: int, pubs, rs, msgs):
+        """n x ecies.Encrypt(BLS12-381 G1 or G2, pubs[i] compressed, msgs[i], sha256.New) with the ephemeral scalars rs[i]
+        (32 bytes big-endian below r); all messages of one length -> ([n] ciphertexts R || C || tag, zero unless OK; n status
+        bytes (0 OK, 1 POINT))"""
+        pl = self.POINT_BYTES[f"bls12381_g{group}"][1]
+        n = len(msgs)
+        length = len(msgs[0]) if n else 0
+        assert len(pubs) == n and len(rs) == n and all(len(m) == length for m in msgs)
+        out, status = bytearray(max(n * (pl + length + 16), 1)), bytearray(n)
+        self._call(f"b2k_bls12381_g{group}_ecies_encrypt", n, b"".join(pubs), b"".join(rs), length, b"".join(msgs), out, status)
+        w = pl + length + 16
+        return [bytes(out[w * i:w * i + w]) for i in range(n)], bytes(status)
+
 
 class Comm:
     """One rank of the sharded MSM (include/b2kyber.h: b2k_comm_*): owns the rank's exchange slab on the engine's device.
